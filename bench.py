@@ -1,11 +1,15 @@
 #!/usr/bin/env python
-"""Benchmark of the DiffuScene denoising hot path on B200 (contract: see the task statement / DESIGN.md 5).
+"""Benchmark of the DiffuScene denoising hot path on H100 (see DESIGN.md 5).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config NAME] [--scaling weak|strong]
+                    [--dump-outputs DIR]
 
 One "step" = one full T-step ancestral DDPM sample of the per-GPU batch: T denoiser forwards + T posterior updates,
 nothing skipped, per-step noise from the in-kernel Philox generator.  `value` = scenes/s with inputs resident in
 HBM; `e2e` = the same through the public sampling API with host (pinned) x_T / condition in and the host result out.
+`--dump-outputs DIR` writes the samples of the last timed step (what a caller of the sampling API receives) as
+DIR/samples.npy (float32, [scenes, N, d]); inputs are seeded, so two builds run with the same arguments can be compared
+output for output.
 Multi-GPU: scenes shard over ranks, no data-path collective (sampling is embarrassingly parallel); `--scaling weak`
 keeps the per-GPU batch, `--scaling strong` splits the config's batch over the ranks; max-over-ranks timing.
 
@@ -57,12 +61,29 @@ W_BYTES_BF16 = 155.35e6          # weights read once per step per GPU (SURVEY 8d
 TEXT_L = 32
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+OP_GEMM, OP_GEMM_GN = 1, 7     # OpKind values of csrc/plan.h
+
+
+def datasheet_peaks():
+    """Dense bf16 tensor rate and HBM3 bandwidth of the H100 SXM data sheet (a 700 W card; a card with a lower power
+    limit clocks lower under sustained load, so `frac` is a lower bound of the share of what that card can reach)."""
+    return 989.0, 3350.0, "H100 SXM data sheet"
+
+
+def dump_outputs(out_dir, arrays, budget=64 << 20):
+    """Write each array as <out_dir>/<name>.npy in float32.  An array larger than its share of the budget is reduced
+    to a fixed, seeded sample of its leading-dimension rows (same rows on every run of the same arguments)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = (budget - (1 << 20)) // max(1, len(arrays))     # headers and row-index files fit in the margin
+    for name, t in arrays.items():
+        a = t.detach().float().cpu()
+        if a.numel() * 4 > share:
+            rows = max(1, share // (4 * max(1, a[0].numel())))
+            idx = torch.randperm(a.shape[0], generator=torch.Generator().manual_seed(0))[:rows].sort().values
+            np.save(os.path.join(out_dir, name + "_rows.npy"), idx.numpy().astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy())
 
 
 class ClockSampler:
@@ -103,8 +124,8 @@ class ClockSampler:
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# CPU arm: the reference's own implementation (oracle/_ref, vendored by oracle/build_ref.py) when it travelled to this
-# box, else the oracle port.  BASELINE.md 3: B = 128 scenes, K = 5 diffusion steps per bench step, all host cores.
+# CPU arm: the reference's own implementation (oracle/_ref, vendored by oracle/build_ref.py) when it is present,
+# else the oracle port.  BASELINE.md 3: B = 128 scenes, K = 5 diffusion steps per bench step, all host cores.
 # ---------------------------------------------------------------------------------------------------------------
 CPU_B, CPU_K = 128, 5
 
@@ -135,7 +156,7 @@ def _yaml_network(cfg_name):
 
 class CpuArm:
     """Times K diffusion steps of B scenes on the host cores through network.sample() of the vendored reference
-    (kind "reference") or, when oracle/_ref did not travel, through the oracle port (kind "port")."""
+    (kind "reference") or, when oracle/_ref is absent, through the oracle port (kind "port")."""
 
     def __init__(self, cfg_name, threads=None):
         self.cfg_name = cfg_name
@@ -290,6 +311,8 @@ def main():
     ap.add_argument("--shape", default=None, help="deprecated alias: real62 -> --config bed_d62, synth97 -> bed_d97")
     ap.add_argument("--fuse", type=int, default=None, help="fuse_level override; default: the engine's")
     ap.add_argument("--profile-ops", action="store_true", help="print the per-op device time table to stderr")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's samples to DIR/samples.npy (float32, at most 64 MB)")
     ap.add_argument("--kv-hoist", type=int, default=1, help="text config: 1 = K/V of the text prefix precomputed once "
                     "per scene (default); 0 = recomputed before every diffusion step (what the reference does)")
     args = ap.parse_args()
@@ -377,6 +400,8 @@ def main():
     ms, launches, out = timed(resident_step, args.steps, args.warmup)
     clk = clocks.stop()
     assert torch.isfinite(out).all()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank), {"samples": out})
     n_e2e = max(1, min(args.steps, 2))
     ms_e2e = None
     if not args.no_e2e:
@@ -387,10 +412,10 @@ def main():
         value = total_scenes * args.steps / (ms / 1000.0)
         ms_per_step = ms / args.steps
         us_per_dstep = ms_per_step * 1000.0 / T
-        peak_tf, peak_gbs, which = measured_peaks()
+        peak_tf, peak_gbs, which = datasheet_peaks()
         flops_per_launch = B * F_SCENE * 1e6            # one diffusion step of one GPU's batch
         achieved_tf = flops_per_launch / (us_per_dstep * 1e-6) / 1e12
-        # which roof binds this per-GPU batch (SURVEY 8d): tensor pipe above ~50 scenes, weight-read HBM below
+        # which roof binds this per-GPU batch: the tensor pipe for large batches, the weight read from HBM below
         t_tensor = flops_per_launch / (peak_tf * 1e12)
         wbytes = W_BYTES_BF16 * (2 if prec == "fp32" else 1)
         t_hbm = wbytes / (peak_gbs * 1e9)
@@ -404,8 +429,8 @@ def main():
             "config": {"workload": "%s, T=%d DDPM sampling, %d scenes/GPU, random-init weights" % (label, T, B),
                        "name": args.config, "scenes_per_gpu": B, "global_batch": total_scenes,
                        "parallelism": "scene-shard x%d (%s scaling)" % (world, args.scaling),
-                       "l2": "per-step working set (activation buffers of %.0f MB each + 63 MB weights) %s the 126 MB L2; "
-                             "no explicit flush" % (B * N_OBJ * 512 * 2 / 1e6, "exceeds" if B * N_OBJ * 512 * 2 * 20 > 126e6 else "fits")},
+                       "l2": "per-step working set (activation buffers of %.0f MB each + 155 MB bf16 weights) exceeds the 50 MB L2; "
+                             "no explicit flush" % (B * N_OBJ * 512 * 2 / 1e6)},
             "denoiser_fwd_us_per_step": us_per_dstep,
             "gpu_launches": int(launches),
             "graph_builds": eng.graph_build_count(),
@@ -417,51 +442,30 @@ def main():
         if hbm_bound:
             ach = wbytes / (us_per_dstep * 1e-6) / 1e9
             res["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs,
-                               "traffic": None, "peak_source": which + " HBM copy bandwidth",
+                               "traffic": None, "peak_source": which + " HBM3 bandwidth",
                                "launch": "one diffusion step over %d scenes: %.2f MB of weights read once (floor %.1f us)"
                                          % (B, wbytes / 1e6, t_hbm * 1e6)}
         else:
             res["roofline"] = {"bound": "tensor", "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s",
-                               "frac": achieved_tf / peak_tf, "traffic": None, "peak_source": which + " bf16 sustained",
+                               "frac": achieved_tf / peak_tf, "traffic": None, "peak_source": which + " dense bf16",
                                "launch": "one diffusion step (CUDA graph of the step program) over %d scenes; "
                                          "algorithmic %.1f MFLOP/scene/step" % (B, F_SCENE)}
-        # dominant kernel: k_gemm_gnt<N>, the channels-on-lanes tcgen05 GEMM that carries the 56 fused conv + GroupNorm
-        # + FiLM + SiLU blocks and the epilogue-bound plain GEMMs.  Timed live with CUDA events around each op of one
-        # eager pass of the step program (launching stream); DRAM traffic from the committed ncu capture.
+        # dominant kernel: k_gemm_wg, the wgmma GEMM that carries every conv / linear layer (plain and fused
+        # conv + GroupNorm + FiLM + SiLU).  Timed live with CUDA events around each op of one eager pass of the step
+        # program (launching stream).
         from diffuscene_b200 import capi
         ops = eng.profile_ops(B) if prec == "bf16" else []
         us_by_name = dict(ops)
-
-        def on_gnt(o):      # mirrors gemm_variant() in csrc/engine.cu
-            if eng.fuse_level < 2 or N_OBJ not in (12, 21) or o["name"] not in us_by_name:
-                return False
-            if o["kind"] == 7:
-                return True
-            k = o["in0"]["k"] + o["in1"]["k"]
-            return o["kind"] == 1 and eng.fuse_level >= 3 and o["N"] % 128 == 0 and (k <= 128 or o["N"] % 256 != 0)
-
-        dom = [o for o in capi.plan_export(eng.cfg)["ops"] if on_gnt(o)] if ops else []
+        dom = [o for o in capi.plan_export(eng.cfg)["ops"] if o["kind"] in (OP_GEMM, OP_GEMM_GN) and o["name"] in us_by_name]
         if dom:
             dom_us = sum(us_by_name[o["name"]] for o in dom)
             dom_flop = sum(2.0 * B * N_OBJ * o["N"] * (o["in0"]["k"] + o["in1"]["k"]) for o in dom)
             res["roofline"]["dominant_kernel"] = {
-                "name": "k_gemm_gnt<%d> (tcgen05 GEMM, output channels on the TMEM lanes; conv+GroupNorm+FiLM+SiLU "
-                        "epilogue, bias-only for the plain launches)" % N_OBJ, "launches_per_step": len(dom),
+                "name": "k_gemm_wg (wgmma GEMM, 128 x 128 tiles; conv+GroupNorm+FiLM+SiLU or bias / activation / "
+                        "residual epilogue)", "launches_per_step": len(dom),
                 "avg_us": dom_us / len(dom), "achieved": dom_flop / (dom_us * 1e-6) / 1e12, "unit": "TFLOP/s",
                 "frac": dom_flop / (dom_us * 1e-6) / 1e12 / peak_tf,
                 "share_of_step": dom_us / max(1e-9, sum(u for _, u in ops))}
-        tpath = os.path.join(ROOT, "profiles", "round2_dram_traffic_%s.json" % args.config)
-        if B == scenes and args.fuse is None and os.path.exists(tpath):
-            with open(tpath) as f:
-                tj = json.load(f)
-            res["roofline"]["traffic"] = tj["step_dram_bytes"]
-            res["roofline"]["traffic_source"] = "profiles/%s (ncu dram__bytes_read+write, one step)" % os.path.basename(tpath)
-            # every instantiation of the kernel that ran in the step (single-CTA and CTA-pair)
-            ks = [v for n, v in tj["kernels"].items() if n.startswith("k_gemm_gnt<%d" % N_OBJ)]
-            if ks and dom:
-                res["roofline"]["dominant_kernel"]["traffic"] = (
-                    sum(k["dram_read_bytes"] + k["dram_write_bytes"] for k in ks) / sum(k["launches"] for k in ks))
-                res["roofline"]["dominant_kernel"]["ncu_share_of_step"] = sum(k["time_ns"] for k in ks) / tj["step_time_ns"]
         if args.profile_ops:
             tot = sum(u for _, u in ops)
             sys.stderr.write("per-op device time (us), total %.1f\n" % tot)

@@ -1,4 +1,4 @@
-"""Build libdiffuscene_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension).
+"""Build libdiffuscene_b200.so in-tree with nvcc for sm_90a (no JIT cache, no torch extension).
 
     python -m diffuscene_b200.build          # or diffuscene_b200.build.build()
 
@@ -18,7 +18,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdiffuscene_b200.so")
 SOURCES = ["engine.cu", "plan.cpp", "pointwise.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_ln.cu", "gemm_attn.cu", "backward.cu", "train.cu"]
 HEADERS = ["common.cuh", "kernels.cuh", "tc_common.cuh", "plan.h", "engine_internal.h", os.path.join("..", "..", "include", "diffuscene_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError("nvcc failed on %s" % src)
         if verbose and out:
             print(out.decode())
-    cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     subprocess.check_call(cmd)
     with open(stamp, "w") as f:
         f.write(digest)

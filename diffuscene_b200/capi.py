@@ -92,9 +92,7 @@ def load(rebuild: bool = False):
         "ds_read_tap": (C.c_int, [H, C.c_char_p, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
         "ds_launch_count": (C.c_int64, [H]),
         "ds_graph_build_count": (C.c_int64, [H]),
-        "ds_gnt_weight_row": (C.c_int32, [C.c_int32]),
         "ds_profile_ops": (C.c_int, [H, C.c_int32, C.c_char_p, C.c_int64, p, C.c_int32]),
-        "ds_test_gemm_trace": (C.c_int, [p, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, C.c_int32, p, p]),
         "ds_test_gemm_bf16": (C.c_int, [C.c_int, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p]),
     }
     for name, (res, args) in sig.items():
@@ -110,8 +108,8 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_set_context_cross", "ds_denoise_forward", "ds_denoise_forward_host", "ds_sample_loop",
             "ds_sample_loop_host", "ds_traj_count", "ds_p_sample_step", "ds_q_sample", "ds_p_losses", "ds_retrieve_objects",
             "ds_train_param_count", "ds_train_step", "ds_train_set_buckets", "ds_train_phase_ms", "ds_sumsq", "ds_adam_step",
-            "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_gnt_weight_row", "ds_profile_ops",
-            "ds_test_gemm_bf16", "ds_test_gemm_trace"]
+            "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
+            "ds_test_gemm_bf16"]
 
 
 class DsError(RuntimeError):

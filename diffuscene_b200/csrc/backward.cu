@@ -133,7 +133,10 @@ template <typename TA, typename TB>
 void launch_gemm_tn(const TA* A, int lda, const TB* B, int ldb, float* D, int ldd, int M, int Ka, int Kb, cudaStream_t s) {
   if (M <= 0 || Ka <= 0 || Kb <= 0) return;
   const int tiles = ((Ka + 63) / 64) * ((Kb + 63) / 64);
-  int splits = (4 * 148 + tiles - 1) / tiles;                   // ~4 blocks per SM
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int splits = (4 * sms + tiles - 1) / tiles;                   // ~4 blocks per SM
   int m_chunk = ((M + splits - 1) / splits + 15) / 16 * 16;
   if (m_chunk < 64) m_chunk = 64;
   splits = (M + m_chunk - 1) / m_chunk;

@@ -1,4 +1,4 @@
-// Shared device helpers for the diffuscene_b200 kernels (sm_100a only).
+// Shared device helpers for the diffuscene_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -64,27 +64,26 @@ static int run_op(ds_handle* h, int idx, int n_scenes, cudaStream_t s) {
     case OP_PACK:
       return DS_ERR_STATE;   // handled by the caller (needs the x pointer)
     case OP_LN_QKV_ATTN: {
-      if (!h->use_tc || !h->atp[idx]) return fail(DS_ERR_STATE, "fused attention op without the tcgen05 backend");
+      if (!h->use_tc || !h->atp[idx]) return fail(DS_ERR_STATE, "fused attention op without the tensor-core backend");
       int e = launch_ln_qkv_attn(h->atp[idx], M, s);
       if (e) return fail(DS_ERR_CUDA, "fused LayerNorm + to_qkv + attention launch '%s' failed: %s", o.name.c_str(),
                          cudaGetErrorString((cudaError_t)e));
       break;
     }
     case OP_GEMM_LN: {
-      if (!h->use_tc || !h->lnp[idx]) return fail(DS_ERR_STATE, "fused LayerNorm op without the tcgen05 backend");
+      if (!h->use_tc || !h->lnp[idx]) return fail(DS_ERR_STATE, "fused LayerNorm op without the tensor-core backend");
       int e = launch_gemm_ln(h->lnp[idx], M, s);
-      if (e) return fail(DS_ERR_CUDA, "tcgen05 GEMM+LayerNorm launch '%s' failed: %s", o.name.c_str(),
+      if (e) return fail(DS_ERR_CUDA, "GEMM + LayerNorm launch '%s' failed: %s", o.name.c_str(),
                          cudaGetErrorString((cudaError_t)e));
       break;
     }
     case OP_GEMM_GN:
-      if (!h->use_tc) return fail(DS_ERR_STATE, "fused GroupNorm op without the tcgen05 backend");
+      if (!h->use_tc) return fail(DS_ERR_STATE, "fused GroupNorm op without the tensor-core backend");
       // fallthrough
     case OP_GEMM: {
       if (h->use_tc) {
-        if (o.kind == OP_GEMM_GN) tc_plan_set_uniform_t(h->tc[idx], h->t_uniform);
         int e = launch_gemm_tc(h->tc[idx], M, s);
-        if (e) return fail(DS_ERR_CUDA, "tcgen05 GEMM launch '%s' failed: %s", o.name.c_str(),
+        if (e) return fail(DS_ERR_CUDA, "tensor-core GEMM launch '%s' failed: %s", o.name.c_str(),
                            cudaGetErrorString((cudaError_t)e));
       } else {
         GemmArgs g;
@@ -166,20 +165,6 @@ static void free_buffers(ds_handle* h) {
   h->cap_scenes = 0;
 }
 
-// which kernel variant a GEMM op runs on (0: row-major tcgen05 kernel, 2: channels-on-lanes GroupNorm, 3: ... plain)
-static int gemm_variant(const ds_handle* h, const Op& o) {
-  if (o.kind == OP_GEMM_GN) return h->gnt ? 2 : 1;
-  // plain GEMMs: the channels-on-lanes kernel wins where the epilogue dominates (K <= 128: to_out) or where the
-  // row-major kernel would fall back to 128-wide tiles (N % 256 != 0: to_qkv); the MMA-bound shapes keep the
-  // row-major kernel, whose 128 x 256 tiles feed the tensor pipe better than 128 x 192 (measured, profiles/)
-  if (o.kind == OP_GEMM && h->gnt_plain && tc_gnt_plain_supported(h->cfg.num_objects, o.N)) {
-    static const int force_all = getenv("DS_GNT_PLAIN_ALL") ? atoi(getenv("DS_GNT_PLAIN_ALL")) : 0;
-    const int K = o.in0.k + (o.in1.buf >= 0 ? o.in1.k : 0);
-    if (force_all || K <= 128 || o.N % 256 != 0) return 3;
-  }
-  return 0;
-}
-
 static int ensure_capacity(ds_handle* h, int n_scenes) {
   if (n_scenes <= 0) return fail(DS_ERR_INVALID, "batch must be positive");
   if (!h->committed) return fail(DS_ERR_STATE, "ds_commit_weights() has not been called");
@@ -229,10 +214,10 @@ static int ensure_capacity(ds_handle* h, int n_scenes) {
         g.M = h->rows_cap; g.N = o.N;
         char err[256] = "";
         h->lnp[i] = ln_plan_create(g, h->rows_cap, err, sizeof err);
-        if (!h->lnp[i]) return fail(DS_ERR_CUDA, "tcgen05 GEMM+LayerNorm plan for op '%s' failed: %s", o.name.c_str(), err);
+        if (!h->lnp[i]) return fail(DS_ERR_CUDA, "GEMM + LayerNorm plan for op '%s' failed: %s", o.name.c_str(), err);
         continue;
       }
-      g.gn = gemm_variant(h, o);
+      g.gn = o.kind == OP_GEMM_GN;
       g.n_obj = n_obj;
       if (o.kind == OP_GEMM_GN) {
         g.film_C = P.C;
@@ -250,7 +235,7 @@ static int ensure_capacity(ds_handle* h, int n_scenes) {
       g.M = h->rows_cap; g.N = o.N; g.act = o.act;
       char err[256] = "";
       h->tc[i] = tc_plan_create(g, h->rows_cap, err, sizeof err);
-      if (!h->tc[i]) return fail(DS_ERR_CUDA, "tcgen05 plan for op '%s' failed: %s", o.name.c_str(), err);
+      if (!h->tc[i]) return fail(DS_ERR_CUDA, "tensor-core GEMM plan for op '%s' failed: %s", o.name.c_str(), err);
     }
   }
   h->cap_scenes = n_scenes;
@@ -344,16 +329,6 @@ extern "C" int ds_commit_weights(ds_handle* h) {
   std::vector<char> host(total, 0);
   std::vector<float> mat;
   std::vector<float> attn_cs_host(P.wmats.size() * 384, 0.f);
-  std::vector<char> gnt_w(P.wmats.size(), 0);       // weight matrices consumed by fused GroupNorm ops
-  std::vector<char> row_major_w(P.wmats.size(), 0);
-  for (const Op& o : P.ops) {
-    if (o.kind == OP_GEMM_LN || o.kind == OP_LN_QKV_ATTN) { row_major_w[o.w] = 1; continue; }
-    if (o.kind != OP_GEMM && o.kind != OP_GEMM_GN) continue;
-    if (gemm_variant(h, o) >= 2) gnt_w[o.w] = 1;
-    else row_major_w[o.w] = 1;
-  }
-  for (size_t i = 0; i < P.wmats.size(); ++i)
-    if (gnt_w[i] && row_major_w[i]) return fail(DS_ERR_STATE, "weight matrix %d is shared by both GEMM layouts", int(i));
   for (size_t i = 0; i < P.wmats.size(); ++i) {
     const WRecipe& r = P.wmats[i];
     mat.assign((size_t)r.N * r.K, 0.f);
@@ -398,11 +373,6 @@ extern "C" int ds_commit_weights(ds_handle* h) {
           attn_cs_host[i * 384 + rr] = float(acc);
         }
       }
-    }
-    if (gnt_w[i]) {      // row order the channels-on-lanes kernel expects (see tc_gnt_row)
-      std::vector<float> pm(mat.size());
-      for (int rr = 0; rr < r.N; ++rr) memcpy(pm.data() + (size_t)rr * r.K, mat.data() + (size_t)tc_gnt_row(rr) * r.K, sizeof(float) * r.K);
-      mat.swap(pm);
     }
     if (h->bf16_mode) to_bf16_host(mat.data(), (uint16_t*)(host.data() + h->w_off[i]), mat.size());
     else memcpy(host.data() + h->w_off[i], mat.data(), mat.size() * 4);
@@ -483,7 +453,7 @@ extern "C" int ds_commit_weights(ds_handle* h) {
 // lifetime
 // ------------------------------------------------------------------------------------------------
 extern "C" const char* ds_last_error(void) { return g_err; }
-extern "C" const char* ds_version(void) { return "diffuscene_b200 0.1 (sm_100a)"; }
+extern "C" const char* ds_version(void) { return "diffuscene_b200 0.1 (sm_90a)"; }
 
 extern "C" int ds_create(const ds_config* cfg, ds_handle** out) {
   if (!cfg || !out) return fail(DS_ERR_INVALID, "null argument");
@@ -497,12 +467,12 @@ extern "C" int ds_create(const ds_config* cfg, ds_handle** out) {
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a only", cfg->device,
+  if (prop.major != 9)
+    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device,
                 prop.major, prop.minor);
   ds_handle* h = new ds_handle();
   h->cfg = *cfg;
-  if (!build_plan(*cfg, false, &h->plan)) {
+  if (!build_plan(h->cfg, false, &h->plan)) {
     int rc = fail(DS_ERR_INVALID, "%s", h->plan.error.c_str());
     delete h;
     return rc;
@@ -511,7 +481,7 @@ extern "C" int ds_create(const ds_config* cfg, ds_handle** out) {
   h->esz = h->bf16_mode ? 2 : 4;
   if (cfg->gemm_backend == DS_GEMM_TCGEN05 && !h->bf16_mode) {
     delete h;
-    return fail(DS_ERR_INVALID, "the tcgen05 backend needs DS_PREC_BF16");
+    return fail(DS_ERR_INVALID, "the tensor-core backend needs DS_PREC_BF16");
   }
   h->use_tc = h->bf16_mode && cfg->gemm_backend != DS_GEMM_SIMT;
   if (h->use_tc) {
@@ -521,10 +491,6 @@ extern "C" int ds_create(const ds_config* cfg, ds_handle** out) {
       return fail(DS_ERR_CUDA, "%s", err);
     }
   }
-  // fuse_level 2: the fused conv + GroupNorm ops use the channels-on-lanes tcgen05 kernel where it applies
-  h->gnt = h->use_tc && cfg->fuse_level >= 2 && tc_gnt_supported(cfg->num_objects, h->plan.C);
-  if (const char* e = getenv("DS_GNT")) h->gnt = h->gnt && atoi(e) != 0;
-  h->gnt_plain = h->gnt && cfg->fuse_level >= 3;
   cudaError_t e = cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) {
     delete h;
@@ -749,7 +715,6 @@ static void model_coefs(ds_handle* h, int t, float* a_x, float* a_o) {
 
 static int step_body(ds_handle* h, const ds_sample_args* a, cudaStream_t s) {
   const Plan& P = h->plan;
-  struct Uni { ds_handle* h; Uni(ds_handle* x) : h(x) { h->t_uniform = 1; } ~Uni() { h->t_uniform = 0; } } uni(h);
   const int B = a->batch, n_obj = h->cfg.num_objects;
   launch_begin_step(h->coef_dev, h->state_dev, h->t_dev, h->x_state, a->partial_dev, a->partial_noise_dev, B, n_obj,
                     P.d, a->partial_dev ? a->num_partial : 0, s);
@@ -917,7 +882,7 @@ extern "C" int ds_sample_loop(ds_handle* h, const ds_sample_args* a, float* out_
   cudaError_t le = cudaGetLastError();
   if (gexec || !stream) CK(cudaStreamSynchronize(s));      // the caller's injected buffers may go away after the call
   if (le != cudaSuccess) return fail(DS_ERR_CUDA, "sampling loop: %s", cudaGetErrorString(le));
-  if (tc_error_flag()) return fail(DS_ERR_CUDA, "tcgen05 pipeline timeout (code %d)", tc_error_flag());
+  if (tc_error_flag()) return fail(DS_ERR_CUDA, "tensor-core GEMM pipeline timeout (code %d)", tc_error_flag());
   return 0;
 }
 
@@ -1019,7 +984,7 @@ extern "C" int ds_p_losses(ds_handle* h, const float* x0_dev, const int64_t* t_d
 }
 
 // ------------------------------------------------------------------------------------------------
-// post-processing: object retrieval (stateless; any sm_100 device)
+// post-processing: object retrieval (stateless; any sm_90 device)
 // ------------------------------------------------------------------------------------------------
 extern "C" int ds_retrieve_objects(const int32_t* class_start_dev, int32_t n_classes, const float* cat_feat_dev,
                                    const float* cat_size_dev, int32_t feat_dim, int32_t size_dim,
@@ -1111,7 +1076,6 @@ extern "C" int ds_read_tap(ds_handle* h, const char* name, float* host_out, int6
 
 extern "C" int64_t ds_launch_count(ds_handle* h) { return h ? h->launches : 0; }
 extern "C" int64_t ds_graph_build_count(ds_handle* h) { return h ? h->graph_builds : 0; }
-extern "C" int32_t ds_gnt_weight_row(int32_t stored_row) { return tc_gnt_row(stored_row); }
 
 extern "C" int ds_profile_ops(ds_handle* h, int32_t batch, char* names_buf, int64_t names_len, float* usec,
                               int32_t cap) {
@@ -1162,56 +1126,6 @@ extern "C" int ds_profile_ops(ds_handle* h, int32_t batch, char* names_buf, int6
   return n;
 }
 
-// Bring-up aid: one tcgen05 GEMM (optionally with the GroupNorm epilogue, n_obj > 0) with per-role cycle counters.
-// trace_host receives [148][8] uint64 (see gemm_tc.cu for the slot meaning); reps launches are timed with events.
-extern "C" int ds_test_gemm_trace(const void* a_dev, const void* w_dev, const float* bias_dev, const void* res_dev,
-                                  void* d_dev, int32_t M, int32_t N, int32_t K, int32_t n_obj, const float* gamma_dev,
-                                  const float* beta_dev, int32_t reps, unsigned long long* trace_host, float* usec) {
-  GemmArgs g;
-  memset(&g, 0, sizeof g);
-  g.a0 = a_dev; g.lda0 = K; g.k0 = K; g.w = w_dev; g.ldw = K; g.bias = bias_dev; g.d = d_dev; g.ldd = N;
-  g.res = res_dev; g.ldres = N; g.M = M; g.N = N;
-  // n_obj < 0: the channels-on-lanes variant (the caller passes the weight rows in tc_gnt_row order)
-  // ... and n_obj < 0 with gamma == NULL: the same kernel as a plain GEMM (act passed in `reps` bits 8.. for the probe)
-  if (n_obj != 0) {
-    g.gn = n_obj < 0 ? (gamma_dev ? 2 : 3) : 1; g.n_obj = n_obj < 0 ? -n_obj : n_obj; g.film_C = N; g.gamma = gamma_dev;
-    g.beta = beta_dev; g.film.mode = FILM_NONE;
-    if (g.gn == 3) { g.act = reps >> 8; reps &= 0xff; }
-  }
-  char err[256] = "";
-  TcGemmPlan* p = tc_plan_create(g, M, err, sizeof err);
-  if (!p) return fail(DS_ERR_CUDA, "%s", err);
-  unsigned long long* tr = nullptr;
-  CK(cudaMalloc(&tr, 256 * 8 * sizeof(unsigned long long)));
-  CK(cudaMemset(tr, 0, 256 * 8 * sizeof(unsigned long long)));
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  int le = 0;
-  for (int i = 0; i < 3; ++i) le |= launch_gemm_tc(p, M, 0);
-  if (le) {       // launch errors are not sticky: without this check a refused launch reads as a 1 us kernel
-    cudaFree(tr);
-    tc_plan_destroy(p);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    return fail(DS_ERR_CUDA, "trace GEMM launch failed: %s", cudaGetErrorString((cudaError_t)le));
-  }
-  cudaEventRecord(e0, 0);
-  for (int i = 0; i < reps; ++i) launch_gemm_tc(p, M, 0);
-  cudaEventRecord(e1, 0);
-  cudaError_t se = cudaDeviceSynchronize();
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  if (usec) *usec = ms * 1000.f / reps;
-  tc_plan_set_trace(p, tr);
-  launch_gemm_tc(p, M, 0);
-  se = cudaDeviceSynchronize();
-  if (trace_host) cudaMemcpy(trace_host, tr, 256 * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-  cudaFree(tr);
-  tc_plan_destroy(p);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  if (se != cudaSuccess) return fail(DS_ERR_CUDA, "trace GEMM failed: %s (code %d)", cudaGetErrorString(se), tc_error_flag());
-  return 0;
-}
-
 extern "C" int ds_test_gemm_bf16(int backend, const void* a_dev, const void* w_dev, const float* bias_dev, void* d_dev,
                                  int32_t M, int32_t N, int32_t K, int32_t act, void* stream) {
   GemmArgs g;
@@ -1228,7 +1142,7 @@ extern "C" int ds_test_gemm_bf16(int backend, const void* a_dev, const void* w_d
     tc_plan_destroy(p);
     if (e) return fail(DS_ERR_CUDA, "launch failed: %s", cudaGetErrorString((cudaError_t)e));
     if (se != cudaSuccess)
-      return fail(DS_ERR_CUDA, "tcgen05 GEMM failed: %s (pipeline code %d)", cudaGetErrorString(se), tc_error_flag());
+      return fail(DS_ERR_CUDA, "tensor-core GEMM failed: %s (pipeline code %d)", cudaGetErrorString(se), tc_error_flag());
     return 0;
   }
   launch_gemm_simt<bf16>(g, false, s);

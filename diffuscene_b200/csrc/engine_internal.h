@@ -39,8 +39,6 @@ struct ds_handle {
   Plan plan;
   bool taps = false;
   bool bf16_mode = false, use_tc = false;
-  bool gnt = false;      // fused GroupNorm convs run the channels-on-lanes kernel (weights stored row-permuted)
-  bool gnt_plain = false;   // ... and so do the plain GEMMs with N % 128 == 0 (fuse_level 3)
   size_t esz = 4;
   cudaStream_t own_stream = nullptr;
   std::map<std::string, std::vector<float>> host_w;
@@ -79,7 +77,6 @@ struct ds_handle {
   int coef_cap = 0;
   StepState* state_dev = nullptr;
   int64_t launches = 0;
-  int t_uniform = 0;          // 1 while every entry of t_dev is the same (inside the sampling loop)
   // instantiated step graph, reused across ds_sample_loop calls whose captured parameters agree (batch, flags,
   // injected-buffer pointers); seed / scene offset / coefficients live in device memory and are not captured
   struct GraphKey {

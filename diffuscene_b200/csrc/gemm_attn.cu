@@ -3,28 +3,25 @@
 // i.e. `Residual(PreNorm(dim, LinearAttention(dim)))` up to (not including) `to_out`
 // (scene_synthesis/networks/denoise_net.py:104-112 PreNorm, :93-102 LayerNorm, :208-233 LinearAttention: qkv = Conv1d(dim,
 // 3 * 128, 1, bias=False); q = softmax over the 32 head channels * 32^-1/2; k = softmax over the tokens;
-// context = k v^T; out = context^T q).  Unfused this was three launches (LayerNorm 25 us, to_qkv GEMM 36 us, core 21 us
-// at 4096 bedroom scenes) with a 50 MB and a 38 MB activation written and re-read in between; k_gemm_ln (gemm_ln.cu)
-// is the other half of the wrapper.
+// context = k v^T; out = context^T q).  Unfused this is three launches (LayerNorm, to_qkv GEMM, core) with two
+// activations written to HBM and re-read in between; k_gemm_ln (gemm_ln.cu) is the other half of the wrapper.
 //
 // The LayerNorm never materialises.  Its gain is folded into the weights when they are packed
 // (W'[n][k] = W[n][k] g[k], ds_commit_weights), and with cs[n] = sum_k W'[n][k]:
 //     to_qkv(LN(x))[row][n] = rstd[row] * ( (x W'^T)[row][n] - mean[row] * cs[n] )
 // so the MMAs run on the raw bf16 x (no extra rounding of a normalised copy) and the per-row statistics are applied
-// to the fp32 accumulator.  The statistics are computed by the epilogue warps from global memory (the same lines the
-// TMA loads are pulling through L2) while the MMAs run.
+// to the fp32 accumulator.  The statistics are computed from global memory (the same lines the TMA loads are pulling
+// through L2) while the first operand tiles are in flight.
 //
-// Tile = SPT whole scenes (10 scenes = 120 token rows for N = 12; UMMA M = 128).  One persistent CTA per SM, 576 threads:
-//   warp 0      TMA producer: per k-block the 128 x 64 x tile and the 384 x 64 W' slab (2 stages x 64 KB)
-//   warp 1      MMA issuer: 2 x tcgen05.mma per k16 step (N = 256 -> TMEM columns 0..255, N = 128 -> 256..383)
-//   warps 2-17  (a) row statistics of the tile (overlaps the MMAs); (b) accumulator -> normalise -> bf16 q | k | v rows
-//               in shared memory ([row][392] bf16: 784-byte rows are conflict-free for ldmatrix and for the 16-byte
-//               row-owner stores), after which TMEM is released and the next tile's MMAs start; (c) the attention core,
-//               one warp per (scene, head), on mma.sync with operands straight from that shared-memory block
-//               (k is soft-maxed in place; rows of the neighbouring scene inside a 16-token MMA tile are masked out of
-//               the v fragments), o written to global memory as packed bf16 pairs.
-// Roof: the 512 KB of operands per tile come from L2 (210 MB per launch at 4096 scenes, ~20 us at the L2 -> SM limit);
-// HBM traffic is x in (50 MB) + o out (12.6 MB).
+// Tile = SPT whole scenes (10 scenes = 120 token rows for N = 12), one CTA per tile, 512 threads = four warpgroups:
+//   mainloop    thread 0 keeps a 2-stage ring of the 128 x 64 x tile and the 384 x 64 W' slab filled by TMA; warpgroup
+//               g multiplies rows 64 (g % 2) .. +63 with W' rows 192 (g / 2) .. +191 (wgmma m64n192k16, 96 fp32
+//               accumulator registers per thread)
+//   epilogue    accumulator -> normalise -> bf16 q | k | v rows in shared memory ([row][392] bf16: 784-byte rows are
+//               conflict-free for ldmatrix), placed over the drained operand ring
+//   core        one warp per (scene, head), on mma.sync with operands straight from that shared-memory block (k is
+//               soft-maxed in place; rows of the neighbouring scene inside a 16-token MMA tile are masked out of the
+//               v fragments), o written to global memory as packed bf16 pairs.
 #include <stdio.h>
 #include <string.h>
 
@@ -33,32 +30,33 @@
 
 namespace ds {
 
+bool tc_encode_2d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems,
+                  uint32_t box_rows, char* err, int err_len);      // gemm_tc.cu
+int* tc_error_flag_dev();
+
 namespace {
 
 constexpr int AT_NQ = 384;                          // q | k | v channels
 constexpr int AT_STAGES = 2;
 constexpr int AT_W_BYTES = AT_NQ * BK * 2;          // 49152
 constexpr int AT_STAGE_BYTES = A_BYTES + AT_W_BYTES;                 // 65536
-constexpr int AT_EPI_W = 16;
-constexpr int AT_THREADS = 64 + AT_EPI_W * 32;
+constexpr int AT_THREADS = 512;
 constexpr int AT_LDS = 392;                         // staging row pitch in bf16 (784 B)
-constexpr int AT_BAR_OFF = AT_STAGES * AT_STAGE_BYTES;               // full[2] empty[2] tfull tempty + tmem slot
+constexpr int AT_BAR_OFF = AT_STAGES * AT_STAGE_BYTES;               // full[2] empty[2]
 constexpr int AT_CS_OFF = AT_BAR_OFF + 64;                           // cs[384] floats
 constexpr int AT_STAT_OFF = AT_CS_OFF + AT_NQ * 4;                   // (mean, rstd)[128]
-constexpr int AT_STG_OFF = AT_STAT_OFF + 128 * 8;
-constexpr uint32_t AT_IDESC_256 = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(256 >> 3) << 17) | (uint32_t(BM >> 4) << 24);
-constexpr uint32_t AT_IDESC_128 = (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(128 >> 3) << 17) | (uint32_t(BM >> 4) << 24);
+constexpr int AT_SMEM = 1024 + AT_STAT_OFF + 128 * 8;
+static_assert(AT_SMEM <= 232448, "shared memory budget exceeded");
 
 template <int NOBJ>
 struct AtCfg {
-  // scenes per tile: 10 x 12 = 120 rows; for N = 21 five scenes (105 rows): six would not leave shared memory for the
-  // 11 masked tail rows of the last scene's second 16-token MMA step
+  // scenes per tile: 10 x 12 = 120 rows; for N = 21 five scenes (105 rows), leaving room for the 11 masked tail rows
+  // of the last scene's second 16-token MMA step
   static constexpr int SPT = (NOBJ == 12) ? 10 : (NOBJ == 21 ? 5 : 128 / NOBJ);
   static constexpr int ROWS = SPT * NOBJ;                            // token rows per tile (<= 128)
   static constexpr int NT = (NOBJ + 15) / 16 * 16;                   // tokens of a scene rounded up to MMA tiles
   static constexpr int STG_ROWS = ROWS + (NT - NOBJ);                // + zeroed tail rows read (masked) by the last scene
-  static constexpr int SMEM = 1024 + AT_STG_OFF + STG_ROWS * AT_LDS * 2;
-  static_assert(SMEM <= 232448, "shared memory budget exceeded");
+  static_assert(STG_ROWS * AT_LDS * 2 <= AT_BAR_OFF, "the q | k | v block lives in the drained operand ring");
 };
 
 struct AtEpi {
@@ -66,8 +64,6 @@ struct AtEpi {
   const float* cs;                  // [384] column sums of the gain-folded, bf16-rounded weights
   bf16* o; int ldo;                 // [M, 128]
   int M, kblocks;
-  uint64_t desc_hi;
-  int uni_issue;           // see tc_common.cuh (DS_TC_UNI)
 };
 
 __device__ __forceinline__ float at_exp2(float x) {
@@ -223,203 +219,138 @@ __global__ void __launch_bounds__(AT_THREADS, 1)
 k_ln_qkv_attn(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w, AtEpi epi, int* err_flag) {
   using Cfg = AtCfg<NOBJ>;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* const base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* const base_ptr = smem_raw + (base - raw);
   const uint32_t bar_base = base + AT_BAR_OFF;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (AT_STAGES + s); };
-  const uint32_t tfull_bar = bar_base + 8u * (2 * AT_STAGES);
-  const uint32_t tempty_bar = bar_base + 8u * (2 * AT_STAGES + 1);
-  const uint32_t tmem_slot = bar_base + 8u * (2 * AT_STAGES + 2);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + AT_BAR_OFF + 8 * (2 * AT_STAGES + 2));
   float* const cs_s = reinterpret_cast<float*>(base_ptr + AT_CS_OFF);
   float2* const stat_s = reinterpret_cast<float2*>(base_ptr + AT_STAT_OFF);
-  bf16* const stg = reinterpret_cast<bf16*>(base_ptr + AT_STG_OFF);
+  bf16* const stg = reinterpret_cast<bf16*>(base_ptr);      // over the operand ring, once the MMAs are done
 
-  const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");     // PDL: the next kernel's prologue may overlap our tail
-  if (warp == 0 && lane == 0) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7, wq = warp & 3;
+  const int m0 = blockIdx.x * Cfg::ROWS;
+  const int rows_here = min(Cfg::ROWS, epi.M - m0);
+  const int nk = epi.kblocks;
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (tid == 0) {
     tma_prefetch_desc(&tm_x);
     tma_prefetch_desc(&tm_w);
     for (int s = 0; s < AT_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), AT_THREADS);
     }
-    mbar_init(tfull_bar, 1);
-    mbar_init(tempty_bar, AT_EPI_W);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  for (int n = tid; n < AT_NQ; n += AT_THREADS) cs_s[n] = __ldg(epi.cs + n);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  asm volatile("griddepcontrol.wait;" ::: "memory");      // nothing above touched memory written by earlier kernels
+  auto issue = [&](int i) {
+    const int s = i % AT_STAGES;
+    const uint32_t sa = base + uint32_t(s * AT_STAGE_BYTES);
+    mbar_expect_tx(full_bar(s), AT_STAGE_BYTES);
+    tma_load_2d(sa, &tm_x, i * BK, m0, full_bar(s));
+    for (int j = 0; j < 3; ++j)      // 128-row boxes
+      tma_load_2d(sa + uint32_t(A_BYTES + j * 128 * 128), &tm_w, i * BK, j * 128, full_bar(s));
+  };
+  if (tid == 0)
+    for (int i = 0; i < AT_STAGES && i < nk; ++i) issue(i);
 
-  const int n_scenes = epi.M / NOBJ;
-  const int num_tiles = (n_scenes + Cfg::SPT - 1) / Cfg::SPT;
-  const int kblocks = epi.kblocks;
-
-  if (warp == 0) {
-    // TMA producer.  UNI: the whole warp walks the loop, one elected lane issues (see tc_common.cuh)
-    auto producer = [&](auto uni_tag) {
-      constexpr bool UNI = decltype(uni_tag)::value;
-      if (!UNI && lane != 0) return;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile * Cfg::ROWS;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u, err_flag, 21);
-          mbar_expect_tx_r<UNI>(full_bar(stage), AT_STAGE_BYTES);
-          const uint32_t sa = base + stage * AT_STAGE_BYTES;
-          tma_load_2d_r<UNI>(sa, &tm_x, kb * BK, m0, full_bar(stage));
+  // ---- LayerNorm statistics of this tile's rows, 8 rows per warp, coalesced 1 KB row reads; the loads of four rows
+  //      are in flight together (one L2 round trip per batch instead of one per row)
 #pragma unroll
-          for (int r3 = 0; r3 < 3; ++r3)      // W' slab: three boxes of 128 rows -> [384 rows][128 B]
-            tma_load_2d_r<UNI>(sa + A_BYTES + r3 * 128 * BK * 2, &tm_w, kb * BK, r3 * 128, full_bar(stage));
-          if (++stage == AT_STAGES) { stage = 0; phase ^= 1u; }
+  for (int rb = 0; rb < 8; rb += 4) {
+    uint4 u[4][2];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int r = warp * 8 + rb + j;
+      u[j][0] = u[j][1] = make_uint4(0u, 0u, 0u, 0u);
+      if (r < rows_here) {
+        const uint4* rp = reinterpret_cast<const uint4*>(epi.x + (int64_t)(m0 + r) * epi.ldx) + lane * 2;
+        u[j][0] = __ldg(rp);
+        u[j][1] = __ldg(rp + 1);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      float s = 0.f, ss = 0.f;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t w4[4] = {u[j][i].x, u[j][i].y, u[j][i].z, u[j][i].w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float a = __uint_as_float(w4[e] << 16), b = __uint_as_float(w4[e] & 0xffff0000u);
+          s += a + b;
+          ss = fmaf(a, a, ss);
+          ss = fmaf(b, b, ss);
         }
       }
-    };
-    if (epi.uni_issue) producer(std::true_type{});
-    else producer(std::false_type{});
-  } else if (warp == 1) {
-    // MMA issuer
-    auto issuer = [&](auto uni_tag) {
-      constexpr bool UNI = decltype(uni_tag)::value;
-      if (!UNI && lane != 0) return;
-      int stage = 0;
-      uint32_t phase = 0, tphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(tempty_bar, tphase ^ 1u, err_flag, 22);
-        tphase ^= 1u;
-        tc_fence_after();
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(full_bar(stage), phase, err_flag, 23);
-          tc_fence_after();
-          const uint32_t sa = base + stage * AT_STAGE_BYTES;
-          const uint64_t adesc = umma_desc(sa, epi.desc_hi);
-          const uint64_t b0 = umma_desc(sa + A_BYTES, epi.desc_hi);
-          const uint64_t b1 = umma_desc(sa + A_BYTES + 256 * BK * 2, epi.desc_hi);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            umma_issue<UNI>(tmem_base, adesc + uint64_t(2 * k), b0 + uint64_t(2 * k), AT_IDESC_256, (kb | k) != 0);
-            umma_issue<UNI>(tmem_base + 256u, adesc + uint64_t(2 * k), b1 + uint64_t(2 * k), AT_IDESC_128, (kb | k) != 0);
-          }
-          umma_arrive<UNI>(empty_bar(stage));
-          if (++stage == AT_STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_arrive<UNI>(tfull_bar);
-      }
-    };
-    if (epi.uni_issue) issuer(std::true_type{});
-    else issuer(std::false_type{});
-  } else {
-    // ---------------- epilogue / core warps ----------------
-    const int ew = warp - 2;                     // 0..15
-    const int q = warp & 3;                      // TMEM lane quadrant of this warp
-    const int part = ew >> 2;                    // which 96 of the 384 columns
-    const int etid = threadIdx.x - 64;
-    auto epi_bar = []() { asm volatile("bar.sync 1, %0;" ::"n"(AT_EPI_W * 32) : "memory"); };
-    for (int n = etid; n < AT_NQ; n += AT_EPI_W * 32) cs_s[n] = __ldg(epi.cs + n);
-    // zero the staging tail once (rows ROWS .. STG_ROWS-1: finite operands for the masked MMA lanes of the last scene)
-    for (int i = etid; i < (Cfg::STG_ROWS - Cfg::ROWS) * AT_LDS / 2; i += AT_EPI_W * 32)
-      reinterpret_cast<uint32_t*>(stg + Cfg::ROWS * AT_LDS)[i] = 0u;
-    const int row_in_tile = q * 32 + lane;
-    uint32_t tphase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = tile * Cfg::ROWS;
-      const int rows_here = min(Cfg::ROWS, epi.M - m0);
-      // ---- (a) LayerNorm statistics of this tile's rows, 8 rows per warp, coalesced 1 KB row reads; the loads of four
-      //      rows are in flight together (one L2 round trip per batch instead of one per row)
-#pragma unroll
-      for (int rb = 0; rb < 8; rb += 4) {
-        uint4 u[4][2];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int r = ew * 8 + rb + j;
-          u[j][0] = u[j][1] = make_uint4(0u, 0u, 0u, 0u);
-          if (r < rows_here) {
-            const uint4* rp = reinterpret_cast<const uint4*>(epi.x + (int64_t)(m0 + r) * epi.ldx) + lane * 2;
-            u[j][0] = __ldg(rp);
-            u[j][1] = __ldg(rp + 1);
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float s = 0.f, ss = 0.f;
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const uint32_t w4[4] = {u[j][i].x, u[j][i].y, u[j][i].z, u[j][i].w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = __uint_as_float(w4[e] << 16), b = __uint_as_float(w4[e] & 0xffff0000u);
-              s += a + b;
-              ss = fmaf(a, a, ss);
-              ss = fmaf(b, b, ss);
-            }
-          }
-          s = warp_sum(s);
-          ss = warp_sum(ss);
-          if (lane == 0) {
-            const float mean = s * (1.0f / 512.0f);
-            const float var = fmaxf(ss * (1.0f / 512.0f) - mean * mean, 0.f);
-            stat_s[ew * 8 + rb + j] = make_float2(mean, rsqrtf(var + 1e-5f));
-          }
-        }
-      }
-      epi_bar();                                  // statistics visible; every warp has left the previous tile's core
-      // ---- (b) accumulator -> q | k | v rows in shared memory
-      mbar_wait(tfull_bar, tphase, err_flag, 24);
-      tphase ^= 1u;
-      tc_fence_after();
-      {
-        const float2 st = stat_s[row_in_tile];
-        const float nmr = -st.x * st.y;           // -mean * rstd
-        bf16* rowp = stg + row_in_tile * AT_LDS + part * 96;
-        uint32_t ra[32];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          tmem_ld32(tmem_base + (uint32_t(q * 32) << 16) + uint32_t(part * 96 + c * 32), ra);
-          if (row_in_tile < Cfg::ROWS) {
-            const float* csp = cs_s + part * 96 + c * 32;
-#pragma unroll
-            for (int g8 = 0; g8 < 4; ++g8) {
-              uint4 o;
-              uint32_t* ow = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int j = g8 * 8 + e * 2;
-                // rstd * (acc - mean * cs) = fma(acc, rstd, (-mean * rstd) * cs)
-                ow[e] = at_pack(fmaf(__uint_as_float(ra[j]), st.y, nmr * csp[j]), fmaf(__uint_as_float(ra[j + 1]), st.y, nmr * csp[j + 1]));
-              }
-              *reinterpret_cast<uint4*>(rowp + c * 32 + g8 * 8) = o;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar);     // accumulator drained: the next tile's MMAs run under the core
-      epi_bar();                                  // all q | k | v rows are in place
-      // ---- (c) attention core: (scene, head) tasks round-robin over the 16 warps
-      const int scenes_here = rows_here / NOBJ;
-      for (int task = ew; task < scenes_here * 4; task += AT_EPI_W) {
-        const int sc = task >> 2, h = task & 3;
-        linattn_core<NOBJ>(stg + sc * NOBJ * AT_LDS, h, epi.o + (int64_t)(m0 + sc * NOBJ) * epi.ldo, epi.ldo, lane);
+      s = warp_sum(s);
+      ss = warp_sum(ss);
+      if (lane == 0) {
+        const float mean = s * (1.0f / 512.0f);
+        const float var = fmaxf(ss * (1.0f / 512.0f) - mean * mean, 0.f);
+        stat_s[warp * 8 + rb + j] = make_float2(mean, rsqrtf(var + 1e-5f));
       }
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
+  // ---- to_qkv on the raw x: warpgroup wg owns rows 64 (wg % 2) + [0, 64), columns 192 (wg / 2) + [0, 192)
+  float acc[96];
+#pragma unroll
+  for (int j = 0; j < 96; ++j) acc[j] = 0.f;
+  for (int i = 0; i < nk; ++i) {
+    const int s = i % AT_STAGES;
+    const uint32_t ph = uint32_t(i / AT_STAGES) & 1u;
+    mbar_wait(full_bar(s), ph, err_flag, 21);
+    const uint32_t sa = base + uint32_t(s * AT_STAGE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      wgmma_m64n192k16(acc, wgmma_desc_sw128(sa + uint32_t((wg & 1) * 64 * 128 + k * 32)),
+                       wgmma_desc_sw128(sa + uint32_t(A_BYTES + (wg >> 1) * 192 * 128 + k * 32)), uint32_t(i | k));
+    wgmma_commit();
+    wgmma_wait0();
+    mbar_arrive(empty_bar(s));
+    if (tid == 0 && i + AT_STAGES < nk) {
+      mbar_wait(empty_bar(s), ph, err_flag, 22);
+      issue(i + AT_STAGES);
+    }
+    __syncwarp();
+  }
+  __syncthreads();      // statistics visible; every MMA has read its operands: the ring becomes the q | k | v block
+
+  // zero the staging tail (rows ROWS .. STG_ROWS-1: finite operands for the masked MMA lanes of the last scene)
+  for (int i = tid; i < (Cfg::STG_ROWS - Cfg::ROWS) * AT_LDS / 2; i += AT_THREADS)
+    reinterpret_cast<uint32_t*>(stg + Cfg::ROWS * AT_LDS)[i] = 0u;
+  // ---- accumulator -> normalised bf16 q | k | v rows.  acc[4 j + 2 h + e]: row r0 + 8 h, column c0 + 8 j + e
+  {
+    const int r0 = (wg & 1) * 64 + wq * 16 + (lane >> 2);
+    const int c0 = (wg >> 1) * 192 + 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
+      if (r >= Cfg::ROWS) continue;
+      const float2 st = stat_s[r];
+      const float nmr = -st.x * st.y;           // -mean * rstd
+      bf16* rowp = stg + r * AT_LDS + c0;
+#pragma unroll
+      for (int j = 0; j < 24; ++j) {
+        const float* csp = cs_s + c0 + 8 * j;
+        // rstd * (acc - mean * cs) = fma(acc, rstd, (-mean * rstd) * cs)
+        *reinterpret_cast<uint32_t*>(rowp + 8 * j) =
+            at_pack(fmaf(acc[4 * j + 2 * h], st.y, nmr * csp[0]), fmaf(acc[4 * j + 2 * h + 1], st.y, nmr * csp[1]));
+      }
+    }
+  }
+  __syncthreads();      // all q | k | v rows are in place
+  // ---- attention core: (scene, head) tasks round-robin over the 16 warps
+  const int scenes_here = rows_here / NOBJ;
+  for (int task = warp; task < scenes_here * 4; task += AT_THREADS / 32) {
+    const int sc = task >> 2, h = task & 3;
+    linattn_core<NOBJ>(stg + sc * NOBJ * AT_LDS, h, epi.o + (int64_t)(m0 + sc * NOBJ) * epi.ldo, epi.ldo, lane);
   }
 }
 
@@ -431,13 +362,8 @@ k_ln_qkv_attn(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ 
 struct AttnQkvPlan {
   CUtensorMap tm_x, tm_w;
   AtEpi epi;
-  int n_obj, num_sms;
+  int n_obj;
 };
-
-bool tc_encode_2d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems,
-                  uint32_t box_rows, char* err, int err_len);      // gemm_tc.cu
-int* tc_error_flag_dev();
-int tc_num_sms();
 
 bool attn_qkv_supported(int n_obj, int C) { return (n_obj == 12 || n_obj == 21) && C == 512; }
 
@@ -452,8 +378,8 @@ AttnQkvPlan* attn_qkv_plan_create(const void* x, int ldx, const void* w, int ldw
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(k_ln_qkv_attn<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, AtCfg<12>::SMEM);
-    cudaFuncSetAttribute(k_ln_qkv_attn<21>, cudaFuncAttributeMaxDynamicSharedMemorySize, AtCfg<21>::SMEM);
+    cudaFuncSetAttribute(k_ln_qkv_attn<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
+    cudaFuncSetAttribute(k_ln_qkv_attn<21>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
     attr_set = true;
   }
   AttnQkvPlan* p = new AttnQkvPlan();
@@ -470,10 +396,7 @@ AttnQkvPlan* attn_qkv_plan_create(const void* x, int ldx, const void* w, int ldw
   p->epi.o = (bf16*)o;
   p->epi.ldo = ldo;
   p->epi.kblocks = K / BK;
-  p->epi.desc_hi = umma_desc_hi_sw128();
-  p->epi.uni_issue = tc_uniform_issue();
   p->n_obj = n_obj;
-  p->num_sms = tc_num_sms();
   return p;
 }
 void attn_qkv_plan_destroy(AttnQkvPlan* p) { delete p; }
@@ -485,11 +408,20 @@ int launch_ln_qkv_attn(const AttnQkvPlan* p, int M, cudaStream_t s) {
   const int spt = p->n_obj == 21 ? AtCfg<21>::SPT : AtCfg<12>::SPT;
   const int tiles = (n_scenes + spt - 1) / spt;
   if (tiles == 0) return 0;
-  const int grid = tiles < p->num_sms ? tiles : p->num_sms;
-  const bool pdl = tc_pdl_enabled(M);
-  if (p->n_obj == 21)
-    return tc_launch(k_ln_qkv_attn<21>, grid, AT_THREADS, AtCfg<21>::SMEM, s, pdl, p->tm_x, p->tm_w, epi, tc_error_flag_dev());
-  return tc_launch(k_ln_qkv_attn<12>, grid, AT_THREADS, AtCfg<12>::SMEM, s, pdl, p->tm_x, p->tm_w, epi, tc_error_flag_dev());
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(tiles);
+  cfg.blockDim = dim3(AT_THREADS);
+  cfg.dynamicSmemBytes = AT_SMEM;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  if (pdl_enabled(0, M)) {
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+  }
+  if (p->n_obj == 21) return (int)cudaLaunchKernelEx(&cfg, k_ln_qkv_attn<21>, p->tm_x, p->tm_w, epi, tc_error_flag_dev());
+  return (int)cudaLaunchKernelEx(&cfg, k_ln_qkv_attn<12>, p->tm_x, p->tm_w, epi, tc_error_flag_dev());
 }
 
 }  // namespace ds

@@ -106,46 +106,33 @@ struct GemmArgs {
   void* d; int ldd;
   const void* res; int ldres;            // optional residual added after the activation
   int M, N, act;
-  // fused GroupNorm(8 groups) + affine + FiLM + SiLU epilogue (tcgen05 backend only)
+  // fused GroupNorm(8 groups) + affine + FiLM + SiLU epilogue (tensor-core backend only)
   int gn;
   int n_obj;
   int film_C;
   const float* gamma;
   const float* beta;
   FilmRef film;
-  // tcgen05 backend: never use the CTA-pair instantiation for this GEMM.  Set by the training step: its GEMMs measured
-  // 4.5 % slower per iteration as pairs (26.8 k vs 28.0 k scenes/s, profiles/round2_final_bench_train_*), unlike the
-  // sampling path's large plain GEMMs
-  int no_pair;
 };
 template <typename T> void launch_gemm_simt(const GemmArgs& g, bool exact, cudaStream_t s);
 // fp32 A/W in, fp32 out (time / context FiLM tables; always fp32)
 void launch_gemm_f32(const GemmArgs& g, cudaStream_t s);
 
-// tcgen05 path: operands described by TMA tensor maps built by the engine (gemm_tc.cu)
+// tensor-core (wgmma) path: operands described by TMA tensor maps built by the engine (gemm_tc.cu)
 struct TcGemmPlan;   // opaque, owns tensor maps
 TcGemmPlan* tc_plan_create(const GemmArgs& g, int rows_capacity, char* err, int err_len);
 void tc_plan_destroy(TcGemmPlan* p);
-void tc_plan_set_film(TcGemmPlan* p, const FilmRef& f);
-void tc_plan_set_trace(TcGemmPlan* p, unsigned long long* trace);
-// Programmatic-dependent-launch policy shared by every launcher of the library (pointwise.cu).  kind 0: tcgen05 GEMM
-// kernels (DS_TC_PDL), kind 1: pointwise kernels (DS_PW_PDL); values 0 off, 1 on, 2 (default) automatic: on when `rows`
-// (tokens of the launch) <= DS_PDL_ROWS (default 32768).  Measured on B200 (profiles/round2_probe_pdl.txt,
-// round2_probe_epi.txt), bedroom N = 12: 1 / 128 / 512 / 1024 / 2048 scenes per GPU gain 8 / 7.5 / 8 / 6 / 3 % (the ~5 us
-// kernel prologue is a large share of each launch), 4096 scenes lose 1.4 % (the chip runs at its power cap there and the
-// early-resident CTAs cost clock).
+void tc_plan_set_film(TcGemmPlan* p, const FilmRef& f);     // FiLM tables may be (re)allocated after planning
+// Programmatic-dependent-launch policy shared by every launcher of the library (pointwise.cu).  kind 0: tensor-core
+// GEMM kernels (DS_TC_PDL), kind 1: pointwise kernels (DS_PW_PDL); values 0 off, 1 on, 2 (default) automatic: on when
+// `rows` (tokens of the launch) <= DS_PDL_ROWS (default 32768), where the kernel prologue is a large share of a launch.
 bool pdl_enabled(int kind, int64_t rows);
 void tc_plan_set_atomic_out(TcGemmPlan* p, float* d32, int ldd, int ksplit);      // split-K, fp32 atomics (dW GEMMs)
 int tc_plan_tiles(const TcGemmPlan* p, int M);
 void tc_plan_set_residual(TcGemmPlan* p, const void* res);      // nullptr: plain store; == output: accumulate in place
-void tc_plan_set_uniform_t(TcGemmPlan* p, int uniform);   // all scenes share one timestep (sampling loop)   // [grid][8] cycle counters   // FiLM tables may be (re)allocated after planning
 int launch_gemm_tc(const TcGemmPlan* p, int M, cudaStream_t s);   // returns 0 or cudaError
 bool tc_runtime_available(char* err, int err_len);
-// GemmArgs.gn == 2 selects the channels-on-lanes GroupNorm GEMM: weight rows must be stored permuted inside every
-// block of 32 output channels (stored row 32 b + l holds channel 32 b + 8 (l % 4) + l / 4)
-bool tc_gnt_supported(int n_obj, int N);
-// GemmArgs.gn == 3: the same kernel as a plain GEMM (bias, activation, residual); same weight row order
-bool tc_gnt_plain_supported(int n_obj, int N);
+int tc_num_sms();      // SMs of the device tc_runtime_available() checked
 // fused GEMM + channel LayerNorm (+ residual) for K <= 128, N = 512 (gemm_ln.cu): GemmArgs.gamma = LayerNorm gain
 struct LnGemmPlan;
 bool ln_gemm_supported(int N, int K);
@@ -159,6 +146,5 @@ AttnQkvPlan* attn_qkv_plan_create(const void* x, int ldx, const void* w, int ldw
                                   int n_obj, int K, int rows_capacity, char* err, int err_len);
 void attn_qkv_plan_destroy(AttnQkvPlan* p);
 int launch_ln_qkv_attn(const AttnQkvPlan* p, int M, cudaStream_t s);
-inline int tc_gnt_row(int stored_row) { const int l = stored_row & 31; return (stored_row & ~31) + 8 * (l & 3) + (l >> 2); }
 
 }  // namespace ds

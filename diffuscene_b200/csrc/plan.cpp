@@ -319,8 +319,8 @@ bool build_plan(const ds_config& cfg, bool no_reuse, Plan* plan) {
   b.no_reuse = no_reuse;
   b.C = C;
   b.train = cfg.train != 0;
-  b.fuse = !b.train && cfg.fuse_level >= 1 && cfg.precision == DS_PREC_BF16 && cfg.gemm_backend != DS_GEMM_SIMT && C % 256 == 0 && C <= 512 &&
-           128 / cfg.num_objects <= 10;   // the fused epilogue's coefficient table holds <= 10 scenes per tile
+  b.fuse = !b.train && cfg.fuse_level >= 1 && cfg.precision == DS_PREC_BF16 && cfg.gemm_backend != DS_GEMM_SIMT && C == 512 &&
+           128 / cfg.num_objects <= 10;   // GroupNorm groups of 64 channels (k_gemm_wg); >= 12 objects per scene
 
   b.fuse_ln = b.fuse && cfg.fuse_level >= 4 && C == 512;
   b.fuse_attn = b.fuse && cfg.fuse_level >= 5 && C == 512 && (cfg.num_objects == 12 || cfg.num_objects == 21);

@@ -25,8 +25,8 @@ enum OpKind {
   OP_LINATTN,       // linear-attention core on qkv [M, 384] -> [M, 128]
   OP_ATTN,          // softmax-attention core
   OP_XATTN,         // cross linear-attention apply (q [M,128] x precomputed text context)
-  OP_GEMM_GN,       // GEMM with the GroupNorm + affine (+FiLM) + SiLU (+res) epilogue fused (tcgen05 only)
-  OP_GEMM_LN,       // GEMM with the channel LayerNorm (gain `gamma`) (+res) epilogue fused (tcgen05 only, fuse_level >= 4)
+  OP_GEMM_GN,       // GEMM with the GroupNorm + affine (+FiLM) + SiLU (+res) epilogue fused (tensor-core backend only)
+  OP_GEMM_LN,       // GEMM with the channel LayerNorm (gain `gamma`) (+res) epilogue fused (fuse_level >= 4; no sm_90a kernel, the engine runs level 1)
   OP_LN_QKV_ATTN,   // channel LayerNorm + to_qkv + linear-attention core in one kernel (fuse_level >= 4, N = 12): the
                     // weight matrix carries the LayerNorm gain (WRecipe::scale_k), out = o [M, 128]
   OP_ACT,           // train mode only: out[:, out_col : out_col + N] = act(in0) (GELU / SiLU as their own op, pre-activation kept)

@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the denoiser and of the diffusion step (sm_100a).
+// Non-GEMM kernels of the denoiser and of the diffusion step (sm_90a).
 //
 // Activation matrices are token-major: row r = scene (r / n_obj), object (r % n_obj); columns are
 // channels.  One warp owns one (scene, group) for GroupNorm, one token for LayerNorm and one
@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(128) k_linattn(const T* __restrict__ qkv, int 
 //     ctx^T[e][d] = sum_n v[n][e] k~[n][d]          (k~ = softmax of k over the scene's tokens)
 //     out^T[e][n] = sum_d ctx^T[e][d] q~[n][d]      (q~ = softmax of q over the 32 head channels, * 32^-1/2)
 // run on mma.sync.m16n8k16 (bf16 operands, fp32 accumulation): 16 HMMAs instead of ~770 FMAs per lane.  These
-// are 32 x 32 x n problems (n <= 32 tokens), far below the 128-row minimum of tcgen05, hence warp-level MMA.
+// are 32 x 32 x n problems (n <= 32 tokens), far below the 128-row tile of the wgmma GEMM, hence warp-level MMA.
 // The accumulator fragments of the first product are re-used directly as the A fragments of the second (the
 // C layout of two adjacent n-tiles is the A layout of one k-tile).
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {

@@ -1,12 +1,9 @@
-// Shared device-side plumbing of the tcgen05 kernels (gemm_tc.cu, gemm_ln.cu): mbarrier / TMA / UMMA / TMEM wrappers
-// around the PTX, the K-major 128B-swizzle descriptors and the MUFU-based activations.  sm_100a only.
+// Shared device-side plumbing of the Hopper tensor-core GEMM (gemm_tc.cu): mbarrier / TMA / wgmma wrappers around
+// the PTX, the K-major 128B-swizzle shared-memory matrix descriptors and the MUFU-based activations.  sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
-
-#include <cstdlib>
-#include <type_traits>
 
 #include "kernels.cuh"
 
@@ -40,16 +37,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a mis-programmed pipeline traps (the launch fails with an error) instead of hanging the GPU.
-// SLEEP_NS > 0 (the single-lane TMA-producer / MMA-issuer roles, which are far off the critical path of an
-// epilogue-bound kernel): back off between polls so that the spinning lane does not take issue slots from the
-// epilogue warps of its SM sub-partition.
-template <int SLEEP_NS = 0>
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* err_flag, int code) {
   if (mbar_try_wait(bar, parity)) return;
   const unsigned long long t0 = clock64();
   unsigned int spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if constexpr (SLEEP_NS > 0) __nanosleep(SLEEP_NS);
     if ((++spins & 0x3FFu) == 0 && clock64() - t0 > WAIT_TIMEOUT_CYCLES) {     // clock read once per 1024 polls
       if (err_flag) atomicExch(err_flag, code);
       __threadfence_system();
@@ -64,267 +56,69 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, int c0, int c1, uint32_t src) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
-               ::"l"(map), "r"(c0), "r"(c1), "r"(src)
-               : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// K-major, 128B-swizzled operand tile as TMA writes it with CU_TENSOR_MAP_SWIZZLE_128B: rows of 128 bytes (64 bf16),
+// 8-row swizzle atoms 1024 bytes apart.  wgmma descriptor: start address >> 4 (bits 0-13), leading byte offset
+// (unused for swizzled K-major, 1), stride byte offset 1024 >> 4 (bits 32-45), layout SWIZZLE_128B = 1 (bits 62-63).
+// Stage buffers are 1024-byte aligned, so the base-offset field stays 0.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row swizzle atoms 1024 bytes apart.
-__host__ __device__ constexpr uint64_t umma_desc_hi_sw128() {
-  return ((uint64_t)1 << 16)                      // leading byte offset (unused for swizzled K-major)
-         | ((uint64_t)(1024 >> 4) << 32)          // stride byte offset between 8-row groups
-         | ((uint64_t)1 << 46)                    // descriptor version (Blackwell)
-         | ((uint64_t)2 << 61);                   // SWIZZLE_128B
-}
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint64_t hi) {
-  return hi | (uint64_t)((smem_addr & 0x3FFFFu) >> 4);   // start address in 16-byte units
-}
-// D(tmem, fp32) (+)= A(smem, bf16) * B(smem, bf16)^T, M = 128, N from the instruction descriptor, K = 16
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x 128] (fp32 registers of the warpgroup) (+)= A[64 x 16] (smem, bf16, K-major) * B[128 x 16]^T (smem, K-major)
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(cta_mask)
-      : "memory");
-}
-// ---- warp-uniform issue (UNI = true) ----------------------------------------------------------------------------
-// The single-thread roles (TMA producer, MMA issuer) can run their loops with the WHOLE warp active: control flow is
-// then warp-uniform, descriptors / barrier addresses / loop counters live in uniform registers, and one elected lane
-// executes each tcgen05 / TMA instruction.  Inside an `if (lane == 0)` region the compiler cannot prove that a single
-// thread is active and wraps every UTCHMMA / UTCBAR / UTMALDG in an ELECT + 5 x R2UR.BROADCAST + BRA.U.ANY waterfall
-// (19 SASS instructions per MMA on the issuing thread; 4 MMAs + commit back to back in the uniform form).  The warp
-// index must be taken through uniform_warp_idx() for this.  elect.sync picks the same lane for the same member mask
-// every time, so the commits track that lane's MMAs.  UNI = false keeps the lane-0 form (A/B switch DS_TC_UNI).
-// host side: the A/B switch shared by every tcgen05 kernel of the library (default: uniform issue)
-inline int tc_uniform_issue() {
-  static const int v = getenv("DS_TC_UNI") ? atoi(getenv("DS_TC_UNI")) : 1;
-  return v;
-}
-inline bool tc_pdl_enabled(int rows) { return pdl_enabled(0, rows); }      // policy: kernels.cuh
-// launch with the optional programmatic-stream-serialization attribute
-template <typename... KArgs, typename... Args>
-inline int tc_launch(void (*kern)(KArgs...), int grid, int threads, size_t smem, cudaStream_t s, bool pdl, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(threads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  if (pdl) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
-  return (int)cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
-__device__ __forceinline__ int uniform_warp_idx() { return __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0); }
-
-template <bool UNI>
-__device__ __forceinline__ void umma_issue(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred p, e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    umma_bf16(d_tmem, a_desc, b_desc, idesc, accumulate);
-  }
-}
-template <bool UNI>
-__device__ __forceinline__ void umma_arrive(uint32_t bar) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
-        : "memory");
-  } else {
-    umma_commit(bar);
-  }
-}
-template <bool UNI>
-__device__ __forceinline__ void umma_arrive_mc(uint32_t bar, uint16_t cta_mask) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-        ::"r"(bar), "h"(cta_mask)
-        : "memory");
-  } else {
-    umma_commit_mc(bar, cta_mask);
-  }
-}
-template <bool UNI>
-__device__ __forceinline__ void mbar_expect_tx_r(uint32_t bar, uint32_t bytes) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes)
-        : "memory");
-  } else {
-    mbar_expect_tx(bar, bytes);
-  }
-}
-template <bool UNI>
-__device__ __forceinline__ void tma_load_2d_r(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n\t}"
-        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar)
-        : "memory");
-  } else {
-    tma_load_2d(dst, map, c0, c1, bar);
-  }
-}
-template <bool UNI>
-__device__ __forceinline__ void tma_load_2d_mc_r(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar,
-                                                 uint16_t cta_mask) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-        " [%0], [%1, {%2, %3}], [%4], %5;\n\t}"
-        ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask)
-        : "memory");
-  } else {
-    tma_load_2d_mc(dst, map, c0, c1, bar, cta_mask);
-  }
-}
-
-// L2 prefetch of a tile a TMA load will fetch later (no shared-memory destination, no barrier)
-template <bool UNI>
-__device__ __forceinline__ void tma_prefetch_2d_r(const CUtensorMap* map, int c0, int c1) {
-  if constexpr (UNI) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n\t}" ::"l"(map), "r"(c0), "r"(c1)
-        : "memory");
-  } else {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
-  }
-}
-
-// ---- CTA pair (cta_group::2): one UMMA of M = 256 spans the two SMs of a cluster of 2 ------------------------------
-// Each CTA keeps its own 128 rows of the M operand and HALF of the N operand's rows in its own shared memory (same
-// offsets in both CTAs); the even ("leader") CTA issues the MMAs for the pair, each CTA's TMEM receives its 128 rows of
-// D.  A shared::cta address used in the shared::cluster window carries the CTA's rank in bit 24, so clearing that bit
-// addresses the leader's copy of a barrier (the convention of the TMA / commit instructions with .cta_group::2).
-static constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-// TMA load into THIS CTA's shared memory whose transaction bytes are counted on the LEADER's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm_elect(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%2, %3}], [%4];\n\t}"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar & PEER_BIT_MASK)
-      : "memory");
-}
-__device__ __forceinline__ void umma_issue_2sm_elect(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                     uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of the pair's MMAs -> one arrival on the barrier at this offset in EVERY CTA of the mask
-__device__ __forceinline__ void umma_arrive_2sm_mc_elect(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-      ::"r"(bar), "h"(cta_mask)
-      : "memory");
-}
-// arrive on the LEADER's copy of a barrier (from either CTA of the pair)
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar & PEER_BIT_MASK) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
+
+// D[64 x 192] (+)= A[64 x 16] * B[192 x 16]^T, same operand conventions as wgmma_m64n128k16
+__device__ __forceinline__ void wgmma_m64n192k16(float (&d)[96], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "%96, %97, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+
 // x * sigmoid(x) = h + h * tanh(h), h = x / 2  (one MUFU op; |rel err| ~ 2^-11, below the bf16 output ulp)
 __device__ __forceinline__ float silu_from_half(float h) {      // argument is x / 2
   float t;
@@ -341,6 +135,5 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   float h = 0.5f * x;
   return fmaf(h, t, h);
 }
-
 
 }  // namespace ds

@@ -139,7 +139,7 @@ struct TrainState {
   float* x_t = nullptr;
   float* loss_parts = nullptr;
   // bf16 mode: tensor-core plans.  Forward GEMMs and dX = dY W (W^T copies `wtarena`, K-major) run the row-major
-  // tcgen05 kernel; dW = dY^T X runs it in split-K mode on transposed copies of dY and X (`trA`, `trB`: [C, rows_cap])
+  // tensor-core kernel; dW = dY^T X runs it in split-K mode on transposed copies of dY and X (`trA`, `trB`: [C, rows_cap])
   bool use_tc = false;
   char* wtarena = nullptr;
   std::vector<TcGemmPlan*> tc_fwd;
@@ -314,7 +314,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
         const int K = P.wmats[o.w].K, Npad = P.wmats[o.w].N;
         GemmArgs g;
         memset(&g, 0, sizeof g);
-        g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
         g.a0 = bp(t->bufs, o.in0.buf, o.in0.col); g.lda0 = P.buf_width[o.in0.buf]; g.k0 = o.in0.k;
         g.a1 = bp(t->bufs, o.in1.buf, o.in1.col); g.lda1 = o.in1.buf >= 0 ? P.buf_width[o.in1.buf] : 0;
         g.k1 = o.in1.buf >= 0 ? o.in1.k : 0;
@@ -324,7 +323,7 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
         g.res = bp(t->bufs, o.res, 0); g.ldres = o.res >= 0 ? P.buf_width[o.res] : 0;
         g.M = t->rows_cap; g.N = o.N; g.act = o.act;
         t->tc_fwd[i] = tc_plan_create(g, t->rows_cap, err, sizeof err);
-        if (!t->tc_fwd[i]) return fail(DS_ERR_CUDA, "train: tcgen05 plan for '%s' failed: %s", o.name.c_str(), err);
+        if (!t->tc_fwd[i]) return fail(DS_ERR_CUDA, "train: tensor-core GEMM plan for '%s' failed: %s", o.name.c_str(), err);
         const Slice* ins[2] = {&o.in0, &o.in1};
         int koff = 0;
         for (int k2 = 0; k2 < 2; ++k2) {
@@ -333,7 +332,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
           // dX = dY W : A = dY [M, N], "weights" = W^T rows [koff, koff + k) of [K, Npad]; accumulates in place
           if (in.buf != t->pack_buf && in.k % 128 == 0 && o.N % 64 == 0) {
             memset(&g, 0, sizeof g);
-            g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
             g.a0 = bp(t->gbufs, o.out, o.out_col); g.lda0 = P.buf_width[o.out]; g.k0 = o.N;
             g.w = (bf16*)(t->wtarena + t->w_off[o.w]) + (size_t)koff * Npad; g.ldw = Npad;
             g.d = bp(t->gbufs, in.buf, in.col); g.ldd = P.buf_width[in.buf];
@@ -345,7 +343,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
           // dW = dY^T X on the transposed copies: A = dY^T [N, rows_cap], "weights" = X^T [k, rows_cap]
           if (in.k % 128 == 0 && o.N % 128 == 0) {
             memset(&g, 0, sizeof g);
-            g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
             g.a0 = t->trA; g.lda0 = t->rows_cap; g.k0 = t->rows_cap;
             g.w = t->trB; g.ldw = t->rows_cap;
             g.d = t->trA; g.ldd = 8;             // placeholder (bf16 output unused in atomic mode)
@@ -353,7 +350,7 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
             t->tc_dw[k2][i] = tc_plan_create(g, o.N, err, sizeof err);
             if (!t->tc_dw[k2][i]) return fail(DS_ERR_CUDA, "train: dW plan for '%s' failed: %s", o.name.c_str(), err);
             const int tiles = tc_plan_tiles(t->tc_dw[k2][i], o.N);
-            int ksplit = std::max(1, 148 / std::max(1, tiles));      // one wave of CTAs: fewer partial sums to reduce
+            int ksplit = std::max(1, 2 * tc_num_sms() / std::max(1, tiles));      // one wave (2 CTAs per SM): fewer partial sums
             const int kblocks = t->rows_cap / 64;
             ksplit = std::min(ksplit, kblocks);
             const int kb_per = (kblocks + ksplit - 1) / ksplit;
@@ -391,7 +388,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
       for (int n0 = 0; n0 < NF; n0 += 4096) {
         const int nn = std::min(4096, NF - n0);
         memset(&g, 0, sizeof g);
-        g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
         g.a0 = t->st_bf; g.lda0 = W4; g.k0 = W4;
         g.w = t->wall_bf + (size_t)n0 * W4; g.ldw = W4;
         g.bias = t->ball + n0;
@@ -403,7 +399,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
         t->tc_film_n0.push_back(n0);
       }
       memset(&g, 0, sizeof g);
-      g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
       g.a0 = t->dfilm_bf; g.lda0 = NF; g.k0 = NF;
       g.w = t->wallT_bf; g.ldw = NF;
       g.d = t->dst_bf; g.ldd = W4;
@@ -412,7 +407,6 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
       if (!t->tc_dst) return fail(DS_ERR_CUDA, "train: d(time embedding) plan failed: %s", err);
       for (size_t i = 0; i < P.time_blocks.size(); ++i) {
         memset(&g, 0, sizeof g);
-        g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
         g.a0 = t->trF + i * (size_t)2 * C * t->Bp; g.lda0 = t->Bp; g.k0 = t->Bp;
         g.w = t->stT; g.ldw = t->Bp;
         g.d = t->trF; g.ldd = 8;
@@ -486,7 +480,6 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
   GemmArgs g;
   auto f32gemm = [&](const float* a, int lda, int K, const float* w, const float* b, float* d, int ldd, int N, int rows) {
     memset(&g, 0, sizeof g);
-    g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
     g.a0 = a; g.lda0 = lda; g.k0 = K; g.w = w; g.ldw = K; g.bias = b; g.d = d; g.ldd = ldd; g.M = rows; g.N = N; g.act = ACT_NONE;
     launch_gemm_f32(g, s);
   };
@@ -540,7 +533,6 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
         break;
       case OP_GEMM: {
         memset(&g, 0, sizeof g);
-        g.no_pair = 1;      // training GEMMs stay single-CTA (kernels.cuh)
         g.a0 = ptr(o.in0.buf, o.in0.col); g.lda0 = ld(o.in0.buf); g.k0 = o.in0.k;
         g.a1 = ptr(o.in1.buf, o.in1.col); g.lda1 = ld(o.in1.buf); g.k1 = o.in1.buf >= 0 ? o.in1.k : 0;
         g.w = t->warena + t->w_off[o.w]; g.ldw = P.wmats[o.w].K;
@@ -550,7 +542,7 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
         g.M = M; g.N = o.N; g.act = o.act;
         if (t->use_tc && t->tc_fwd[&o - &P.ops[0]]) {
           int e = launch_gemm_tc(t->tc_fwd[&o - &P.ops[0]], M, s);
-          if (e) return fail(DS_ERR_CUDA, "train: tcgen05 GEMM '%s' failed: %s", o.name.c_str(), cudaGetErrorString((cudaError_t)e));
+          if (e) return fail(DS_ERR_CUDA, "train: tensor-core GEMM '%s' failed: %s", o.name.c_str(), cudaGetErrorString((cudaError_t)e));
         } else {
           launch_gemm_simt<T>(g, true, s);
         }
@@ -677,7 +669,7 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
       k_dfilm_prepare<<<grid, block, 0, s>>>(df, NF, t->dfilm_bf + (size_t)i * 2 * C, NF, t->trF + (size_t)i * 2 * C * t->Bp, t->Bp,
                                              B, 2 * C, G(P.time_blocks[i] + ".mlp.1.bias"));
       const int tiles = tc_plan_tiles(t->tc_dwf[i], 2 * C), kblocks = t->Bp / 64;
-      int ksplit = std::max(1, std::min(148 / std::max(1, tiles), kblocks));
+      int ksplit = std::max(1, std::min(2 * tc_num_sms() / std::max(1, tiles), kblocks));
       const int kb_per = (kblocks + ksplit - 1) / ksplit;
       ksplit = (kblocks + kb_per - 1) / kb_per;
       tc_plan_set_atomic_out(t->tc_dwf[i], G(P.time_blocks[i] + ".mlp.1.weight"), W4, ksplit);

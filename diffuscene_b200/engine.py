@@ -31,21 +31,21 @@ class DenoiserEngine:
     def __init__(self, spec: NetSpec, num_objects: int, num_timesteps: int, precision: str = "bf16",
                  gemm_backend: str = "auto", device: int = 0, fuse_level: Optional[int] = None):
         if not torch.cuda.is_available():
-            raise RuntimeError("diffuscene_b200 needs a CUDA device (B200, sm_100a); there is no CPU path")
+            raise RuntimeError("diffuscene_b200 needs a CUDA device (H100, sm_90a); there is no CPU path")
         self.lib = capi.load()
         self.spec = spec
         self.num_objects = num_objects
         self.num_timesteps = num_timesteps
         self.precision = precision
         self.device = torch.device("cuda", device)
-        if fuse_level is None:      # fused GEMM epilogues exist for the tcgen05 path only
-            # 2: conv + GroupNorm GEMMs with the channels on the TMEM lanes where the library supports the shape
-            # (N = 12 objects), the row-major fused kernel (level 1) otherwise
-            # 3: ... and the epilogue-bound plain GEMMs (to_qkv, to_out) on the same kernel
+        if fuse_level is None:      # fused GEMM epilogues exist for the tensor-core path only
+            # 1: every conv + GroupNorm + FiLM + SiLU Block is one GEMM with the GroupNorm epilogue (k_gemm_wg)
             # 4: ... and to_out + LayerNorm + residual of the attention wrappers as one kernel (k_gemm_ln)
-            # 5: ... and LayerNorm + to_qkv + linear-attention core as one kernel (k_ln_qkv_attn, N = 12)
+            # 5: ... and LayerNorm + to_qkv + linear-attention core as one kernel (k_ln_qkv_attn, N = 12 or 21)
             fuse_level = 5 if (precision == "bf16" and gemm_backend != "simt") else 0
-        self.fuse_level = fuse_level
+        # levels 2 and 3 named the channels-on-tensor-memory-lanes GEMM of the sm_100a build; the library runs the
+        # level-1 program for them, and this attribute reports the level that runs
+        self.fuse_level = 1 if fuse_level in (2, 3) else fuse_level
         self.cfg = capi.make_config(spec, num_objects, num_timesteps, _PREC[precision], _BACKEND[gemm_backend],
                                     device, fuse_level)
         h = C.c_void_p()

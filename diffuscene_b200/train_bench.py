@@ -65,7 +65,7 @@ def run_reference_train(args):
             with contextlib.redirect_stdout(io.StringIO()):
                 return train_on_batch(net, opt, sp, cfg)
     else:
-        raise SystemExit(json.dumps({"impl": "reference", "unavailable": "oracle/_ref did not travel; the oracle has no training loop"}))
+        raise SystemExit(json.dumps({"impl": "reference", "unavailable": "oracle/_ref is not vendored; the oracle has no training loop"}))
     ts = []
     for i in range(args.warmup + args.steps):
         t0 = time.perf_counter()
@@ -86,6 +86,8 @@ def run_reference_train(args):
 
 
 def run_train_bench(args):
+    if args.dump_outputs:
+        raise SystemExit("--dump-outputs covers the sampling configs; the training bench has no sample output")
     if args.impl == "reference":
         return run_reference_train(args)
     import torch.distributed as dist
@@ -97,7 +99,7 @@ def run_train_bench(args):
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     sys.path.insert(0, ROOT)
-    from bench import ClockSampler, measured_peaks
+    from bench import ClockSampler, datasheet_peaks
     from scene_synthesis.networks import build_network, optimizer_factory
     cfg = _config("/tmp/ds_b200_train_stats_%d.json" % rank)
     prec = args.precision or "bf16"
@@ -162,7 +164,7 @@ def run_train_bench(args):
         total = B * world
         value = total * args.steps / (ms / 1000.0)
         ms_per_step = ms / args.steps
-        peak_tf, _, which = measured_peaks()
+        peak_tf, _, which = datasheet_peaks()
         ach = B * F_TRAIN_MFLOP * 1e6 / (ms_per_step * 1e-3) / 1e12
         assert last == last, "loss is NaN"
         print(json.dumps({
@@ -172,14 +174,14 @@ def run_train_bench(args):
             "config": {"workload": "DDP training uncond living room N=21 d=65 (BASELINE configs[4]), Adam, loss_separate + "
                                    "loss_iou, clip 10, %d scenes/GPU, random-init weights" % B, "name": "train",
                        "scenes_per_gpu": B, "global_batch": total, "parallelism": "data-parallel x%d (%s scaling)" % (world, args.scaling),
-                       "l2": "activations kept for the backward pass (%.1f GB) exceed the 126 MB L2; no explicit flush"
+                       "l2": "activations kept for the backward pass (%.1f GB) exceed the 50 MB L2; no explicit flush"
                              % (190 * B * N * 512 * (2 if prec == "bf16" else 4) / 1e9)},
             "gpu_launches": int(launches), "clocks": clk, "last_loss": last,
             "phases_ms": phases, "allreduce_ms": ar_ms, "allreduce_share": ar_ms / ms_per_step if ms_per_step else None,
             "e2e": {"value": total * n_e2e / (ms_e2e / 1000.0), "unit": "scenes/s",
                     "h2d_bytes_per_step": int(sum(v.numel() * 4 for v in host.values())), "d2h_bytes_per_step": 4},
             "roofline": {"bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": ach / peak_tf,
-                         "traffic": None, "peak_source": which + " bf16 sustained",
+                         "traffic": None, "peak_source": which + " dense bf16",
                          "launch": "one optimizer iteration over %d scenes; algorithmic 3 x 1455.7 MFLOP/scene" % B}}))
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * diffuscene_b200 -- C ABI of the B200-native DiffuScene denoising hot path.
+ * diffuscene_b200 -- C ABI of the H100-native (sm_90a) DiffuScene denoising hot path.
  *
  * The reference (tangjiapeng/DiffuScene) is pure Python/PyTorch and has no FFI of its own; this
  * header is the boundary a maintainer binds with ctypes (see INTEGRATION.md).  Each entry point
@@ -34,7 +34,7 @@ typedef struct ds_handle ds_handle;
 enum ds_status {
   DS_OK = 0,
   DS_ERR_INVALID = -1,      /* bad argument / unsupported configuration            */
-  DS_ERR_NO_DEVICE = -2,    /* no CUDA device or not sm_100                        */
+  DS_ERR_NO_DEVICE = -2,    /* no CUDA device or not sm_90                         */
   DS_ERR_CUDA = -3,         /* a CUDA runtime / driver call failed                 */
   DS_ERR_STATE = -4,        /* call order violated (weights / schedule / context)  */
   DS_ERR_MISSING_WEIGHT = -5
@@ -42,13 +42,13 @@ enum ds_status {
 
 enum ds_precision {
   DS_PREC_FP32 = 0,   /* parity mode: fp32 storage + fp32 FMA GEMMs (rtol 1e-3 / atol 1e-4 vs reference) */
-  DS_PREC_BF16 = 1    /* throughput mode: bf16 storage, tcgen05 tensor-core GEMMs, fp32 accumulate/norms */
+  DS_PREC_BF16 = 1    /* throughput mode: bf16 storage, wgmma tensor-core GEMMs, fp32 accumulate/norms */
 };
 
 enum ds_gemm_backend {
-  DS_GEMM_AUTO = 0,   /* tcgen05 for bf16, SIMT for fp32 */
+  DS_GEMM_AUTO = 0,   /* tensor cores (wgmma) for bf16, SIMT for fp32 */
   DS_GEMM_SIMT = 1,   /* CUDA-core GEMM for either precision (debug / cross-check) */
-  DS_GEMM_TCGEN05 = 2
+  DS_GEMM_TCGEN05 = 2 /* the tensor-core (wgmma) backend; the name is kept for ABI compatibility */
 };
 
 enum ds_mean_type { DS_MEAN_EPS = 0, DS_MEAN_X0 = 1, DS_MEAN_V = 2 };
@@ -69,12 +69,15 @@ typedef struct ds_config {
   int32_t precision;        /* ds_precision                                            */
   int32_t gemm_backend;     /* ds_gemm_backend                                         */
   int32_t device;           /* CUDA device ordinal                                     */
-  int32_t fuse_level;       /* 0: one kernel per op; 1: fused GEMM epilogues; 2: + the
-                               channels-on-lanes conv+GroupNorm GEMM where supported;
-                               3: + epilogue-bound plain GEMMs on that kernel;
-                               4: + to_out + LayerNorm + residual of the attention wrappers
-                                  as one GEMM with a LayerNorm epilogue;
-                               5: + LayerNorm + to_qkv + linear-attention core as one kernel (N = 12) */
+  int32_t fuse_level;       /* 0: one kernel per op; 1: conv + GroupNorm + FiLM + SiLU blocks
+                                  as one GEMM with a GroupNorm epilogue;
+                               2, 3: the channels-on-tensor-memory-lanes GEMM variants of the
+                                  sm_100a build; sm_90a has no tensor memory, so these levels
+                                  run the level-1 program;
+                               4: level 1 + to_out + LayerNorm + residual of the attention
+                                  wrappers as one GEMM with a LayerNorm epilogue;
+                               5: level 4 + LayerNorm + to_qkv + linear-attention core as one
+                                  kernel (N = 12 or 21) */
   int32_t train;            /* 1: training step program -- one op per reference layer (no fused epilogues, activations
                                as their own ops), every intermediate kept for the backward pass (ds_train_*)   */
   int32_t reserved[6];
@@ -242,9 +245,6 @@ DS_API int64_t ds_launch_count(ds_handle* h);
 /* How many times ds_sample_loop had to capture + instantiate its step graph (it is cached across calls whose
  * batch / flags / injected-buffer pointers agree; seeds and shard offsets live in device memory). */
 DS_API int64_t ds_graph_build_count(ds_handle* h);
-/* Weight layout of the channels-on-lanes GEMM (fuse_level >= 2): the output channel whose weights are stored in row
- * `stored_row` of a packed [N, K] matrix.  Host-only (no device needed); identity for the row-major kernels. */
-DS_API int32_t ds_gnt_weight_row(int32_t stored_row);
 /* Per-op device time of one forward (CUDA events around each op; profiling aid, not a bench number).
  * Writes up to `cap` entries of (name, microseconds). Returns op count. */
 DS_API int ds_profile_ops(ds_handle* h, int32_t batch, char* names_buf, int64_t names_len, float* usec, int32_t cap);
@@ -252,15 +252,6 @@ DS_API int ds_profile_ops(ds_handle* h, int32_t batch, char* names_buf, int64_t 
  * backend. Device pointers. */
 DS_API int ds_test_gemm_bf16(int backend, const void* a_dev, const void* w_dev, const float* bias_dev, void* d_dev,
                       int32_t M, int32_t N, int32_t K, int32_t act, void* stream);
-
-/* Bring-up / profiling aid: one tcgen05 GEMM (GroupNorm epilogue when n_obj > 0) timed with CUDA events over
- * `reps` launches, plus per-role cycle counters of one traced launch: trace_host[256][8] uint64.
- * n_obj < 0 selects the channels-on-lanes kernel for |n_obj| objects per scene; the caller then passes the weight
- * rows in that kernel's order (stored row 32b+l = channel 32b + 8(l%4) + l/4).  With gamma_dev == NULL it runs as a
- * plain GEMM whose activation (0 none, 1 GELU, 2 SiLU) travels in bits 8.. of `reps`. */
-DS_API int ds_test_gemm_trace(const void* a_dev, const void* w_dev, const float* bias_dev, const void* res_dev,
-                              void* d_dev, int32_t M, int32_t N, int32_t K, int32_t n_obj, const float* gamma_dev,
-                              const float* beta_dev, int32_t reps, unsigned long long* trace_host, float* usec);
 
 #ifdef __cplusplus
 }

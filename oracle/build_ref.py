@@ -1,14 +1,15 @@
 """ORACLE build recipe (test / bench infrastructure, never imported by the product): vendor the reference's own
-implementation of the path into oracle/_ref/ so that it can travel to the GPU box and be timed there as the CPU arm.
+implementation of the path into oracle/_ref/ so that bench.py can time it on the host cores as the CPU arm.
 
-    python oracle/build_ref.py            # needs /root/reference (authoring container); writes oracle/_ref/ only
+    python oracle/build_ref.py            # reads the reference checkout at $DS_REFERENCE_ROOT; writes oracle/_ref/ only
 
 The reference is Python: "building" it means copying the import closure of `scene_synthesis.networks`
 (networks/{__init__, denoise_net, diffusion_ddpm, diffusion_scene_layout_ddpm, loss, feature_extractors,
 frozen_batchnorm}.py, stats_logger.py, the package __init__) byte for byte from where the sources lie, plus empty
 stand-ins for the four modules the reference imports and does not use on this path and that this image lacks
 (`tkinter`, `clip`: stray IDE imports / an optional text encoder, SURVEY 8c).  oracle/_ref/ is git-ignored (history
-stays free of reference sources) and is NOT gpurun-ignored.  A MANIFEST with sha256 of every copied file is written
+stays free of reference sources).  Without a reference checkout build() does nothing and the bench times the oracle
+port instead.  A MANIFEST with sha256 of every copied file is written
 so that a run can state exactly what it timed.
 """
 import hashlib
@@ -30,7 +31,7 @@ STUBS = {"tkinter/__init__.py": "", "tkinter/messagebox.py": "NO = 0\n", "tkinte
 
 def build(verbose=True):
     if not os.path.isdir(SRC):
-        return None                         # GPU box: use the prebuilt copy (or fall back to the oracle port)
+        return None                         # keep a copy vendored earlier, if any (else the bench uses the oracle port)
     if os.path.isdir(DST):
         shutil.rmtree(DST)
     manifest = {}

@@ -34,7 +34,7 @@ def main(argv):
     p.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
     args = p.parse_args(argv)
     if not torch.cuda.is_available():
-        raise RuntimeError("generate_diffusion.py needs a CUDA device (B200); there is no CPU path")
+        raise RuntimeError("generate_diffusion.py needs a CUDA device (H100); there is no CPU path")
     device = torch.device("cuda:0")
     os.makedirs(args.output_directory, exist_ok=True)
     torch.manual_seed(args.seed)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Training entry point (reference scripts/train_diffusion.py:27-255) on the B200-native network.
+"""Training entry point (reference scripts/train_diffusion.py:27-255) on the H100-native network.
 
 Same positional arguments, flags, experiment-directory layout and checkpoint files.  The 3D-FRONT data layer is
 absent in this sandbox, so `--synthetic` (the default) feeds scenes from diffuscene_b200.synthetic with the same
@@ -40,7 +40,7 @@ def main(argv):
     np.random.seed(args.seed)
     torch.manual_seed(np.random.randint(np.iinfo(np.int32).max))
     if not torch.cuda.is_available():
-        raise RuntimeError("train_diffusion.py needs a CUDA device (B200); there is no CPU path")
+        raise RuntimeError("train_diffusion.py needs a CUDA device (H100); there is no CPU path")
     torch.cuda.manual_seed_all(np.random.randint(np.iinfo(np.int32).max))
     device = torch.device("cuda:0")
 

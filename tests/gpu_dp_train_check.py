@@ -1,4 +1,4 @@
-"""Run under torchrun with 2 ranks on a multi-GPU box (scripts/gpu_run.sh dp2):
+"""Run under torchrun with 2 ranks on a machine with two GPUs (python -m torch.distributed.run --nproc-per-node 2):
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 tests/gpu_dp_train_check.py
 Data-parallel native training on NCCL: every rank takes its shard through model.get_loss().backward() (native backward,
 bucketed all-reduce overlapped with it) and the averaged gradient must equal the gradient of the full batch computed

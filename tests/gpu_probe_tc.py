@@ -1,16 +1,13 @@
-"""Bring-up probe for the tcgen05 GEMM (run on the GPU box, not a pytest test): structured inputs whose
-output reveals operand-layout / descriptor mistakes; dumps results under gpurun_out/ for offline reading."""
+"""Bring-up probe for the tensor-core GEMM (run by hand on a GPU, not a pytest test): structured inputs whose
+output reveals operand-layout / descriptor mistakes."""
 import os
 import sys
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from diffuscene_b200 import capi   # noqa: E402
 
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
-os.makedirs(OUT, exist_ok=True)
 lib = capi.load()
 tag = sys.argv[1] if len(sys.argv) > 1 else "default"
 
@@ -27,7 +24,6 @@ def run(a, w, name):
     ref = a.float() @ w.float().t()
     err = (d.float() - ref).abs().max().item()
     print("%s [%s]: M=%d N=%d K=%d max_err=%.4g ref_max=%.4g" % (name, tag, M, N, K, err, ref.abs().max().item()))
-    np.save(os.path.join(OUT, "probe_%s_%s.npy" % (tag, name)), d.float().cpu().numpy())
     return err
 
 

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), name
     assert sorted(declared) == sorted(capi.EXPORTED)
-    assert b"sm_100a" in lib.ds_version()
+    assert b"sm_90a" in lib.ds_version()
 
 
 @pytest.mark.parametrize("name", list(CASES))
@@ -67,23 +67,3 @@ def test_no_cpu_fallback():
     with pytest.raises(RuntimeError):
         DenoiserEngine(spec, 12, 1000)
 
-
-def test_channels_on_lanes_weight_row_order():
-    """ds_gnt_weight_row (host-only): the row permutation ds_commit_weights applies to the convs of the fused GroupNorm
-    blocks.  Checked against a model of the data path it exists for: TMEM lane l of a 32-lane quadrant belongs to
-    thread l of an epilogue warp; the warp packs (token j, token j+1) pairs and stores them with stmatrix.trans, where
-    thread l contributes column l // 4 of rows 2 (l % 4) + {0, 1} of an 8 x 8 b16 matrix whose row 2 c + e is the
-    16-byte chunk c (8 channels) of token j + e in a [token][32 channel] block.  The block is channel-contiguous iff
-    the thread on lane l holds channel 8 (l % 4) + l // 4."""
-    lib = capi.load()
-    rows = [lib.ds_gnt_weight_row(r) for r in range(256)]
-    for b in range(0, 256, 32):
-        blk = rows[b:b + 32]
-        assert sorted(blk) == list(range(b, b + 32))                  # a permutation inside every block of 32
-    block = {}                                                          # (token e, channel slot) -> channel
-    for l in range(32):
-        chunk, col = l % 4, l // 4                                      # stmatrix.trans: rows 2 chunk + e, column col
-        for e in (0, 1):
-            block[(e, 8 * chunk + col)] = rows[l]                       # slot = position inside the 64-byte token row
-    for e in (0, 1):
-        assert [block[(e, s)] for s in range(32)] == list(range(32))   # channels land in order: coalesced rows
