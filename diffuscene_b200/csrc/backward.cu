@@ -7,6 +7,7 @@
 //   Block           k_gn_bwd: GroupNorm(8) + affine + FiLM + SiLU (+ residual passthrough) in one pass per (scene, group)
 //   LayerNorm       k_ln_bwd
 //   LinearAttention k_linattn_bwd, Attention k_softattn_bwd (one warp per (scene, head), everything in shared memory)
+//   LinearAttentionCross k_xattn_apply_bwd (object side); its text side, k_xattn_prepare_bwd, is in pointwise.cu
 //   loss            k_p_losses_bwd: d(loss)/d(model output) for the MSE terms and the IoU regulariser
 //   weights         k_ws_unpack: packed-matrix gradients -> named tensors through the weight-standardisation adjoint
 //   optimizer       k_adam, k_sumsq (global gradient norm for clip_grad_norm_)
@@ -655,6 +656,62 @@ void launch_linattn_bwd(const T* qkv, int ld, const T* dout, int ldo, T* dqkv, i
   if (n_scenes > 0) k_linattn_bwd<T><<<n_scenes * 4, 32, 0, s>>>(qkv, ld, dout, ldo, dqkv, lddq, n_scenes, N);
 }
 
+// LinearAttentionCross, object side (denoise_net.py:261-297; forward: k_xattn_apply): one CTA per scene, one warp per
+// head, lane = channel.  Per object n, with p = softmax over the 32 channels of q and q^ = s p:
+//   dq^[d] = sum_e ctx[d][e] dO[e]      dctx[d][e] += q^[d] dO[e]      dq = s p (dq^ - sum_d' p[d'] dq^[d'])
+// dctx is summed over the scene's objects in registers (lane = d, one row each) and stored once: no atomics.
+template <typename T>
+__global__ void __launch_bounds__(128) k_xattn_apply_bwd(const T* __restrict__ q, int ldq, const T* __restrict__ dout,
+                                                         int ldo, const float* __restrict__ ctx, T* __restrict__ dq,
+                                                         int lddq, int accumulate, float* __restrict__ dctx, int n) {
+  __shared__ float tr[4][32][33];      // per head: ctx (and at the end dctx) transposed between lane = e and lane = d
+  const int lane = threadIdx.x & 31, h = threadIdx.x >> 5;
+  const int scene = blockIdx.x;
+  const float* cx = ctx + ((int64_t)scene * 4 + h) * 1024;
+#pragma unroll 8
+  for (int d = 0; d < 32; ++d) tr[h][d][lane] = cx[d * 32 + lane];
+  __syncwarp();
+  float cr[32], acc[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) {
+    cr[e] = tr[h][lane][e];
+    acc[e] = 0.f;
+  }
+  const int64_t row0 = (int64_t)scene * n;
+  const float scale = 0.17677669529663687f;      // 32^-1/2
+  for (int r = 0; r < n; ++r) {
+    const float qv = ldf(q + (row0 + r) * ldq + h * 32 + lane);
+    const float m = warp_max(qv);
+    const float ex = expf(qv - m);
+    const float p = ex / warp_sum(ex);
+    const float qh = p * scale;
+    const float dov = ldf(dout + (row0 + r) * ldo + h * 32 + lane);
+    float dqh = 0.f;
+#pragma unroll
+    for (int e = 0; e < 32; ++e) {
+      const float de = __shfl_sync(0xffffffffu, dov, e);
+      dqh = fmaf(cr[e], de, dqh);
+      acc[e] = fmaf(qh, de, acc[e]);
+    }
+    const float g = scale * p * (dqh - warp_sum(p * dqh));
+    T* pq = dq + (row0 + r) * lddq + h * 32 + lane;
+    stf(pq, accumulate ? ldf(pq) + g : g);
+  }
+  __syncwarp();
+#pragma unroll
+  for (int e = 0; e < 32; ++e) tr[h][lane][e] = acc[e];
+  __syncwarp();
+  float* o = dctx + ((int64_t)scene * 4 + h) * 1024;
+#pragma unroll 8
+  for (int d = 0; d < 32; ++d) o[d * 32 + lane] = tr[h][d][lane];
+}
+template <typename T>
+void launch_xattn_apply_bwd(const T* q, int ldq, const T* dout, int ldo, const float* ctx, T* dq, int lddq,
+                            int accumulate, float* dctx, int n_scenes, int n_obj, cudaStream_t s) {
+  if (n_scenes > 0)
+    k_xattn_apply_bwd<T><<<n_scenes, 128, 0, s>>>(q, ldq, dout, ldo, ctx, dq, lddq, accumulate, dctx, n_obj);
+}
+
 // Attention (denoise_net.py:237-259): sim[i][j] = scale * sum_d q[d][i] k[d][j], attn = softmax_j, out[i][d] = sum_j attn[i][j] v[j][d]
 template <typename T>
 __global__ void __launch_bounds__(32) k_softattn_bwd(const T* __restrict__ qkv, int ld, const T* __restrict__ dout, int ldo,
@@ -1029,6 +1086,8 @@ void launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float 
   template void launch_ln_bwd<T>(const T*, int, const T*, int, T*, int, int, T*, int, int, const float*, float*, int, \
                                  int, cudaStream_t);                                                                  \
   template void launch_linattn_bwd<T>(const T*, int, const T*, int, T*, int, int, int, cudaStream_t);                 \
+  template void launch_xattn_apply_bwd<T>(const T*, int, const T*, int, const float*, T*, int, int, float*, int, int, \
+                                          cudaStream_t);                                                              \
   template void launch_softattn_bwd<T>(const T*, int, const T*, int, T*, int, int, int, cudaStream_t);                \
   template void launch_p_losses_bwd<T>(const float*, const float*, const float*, const T*, int, const int64_t*,       \
                                        const float*, const float*, const float*, const float*, const float*,          \

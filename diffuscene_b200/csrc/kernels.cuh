@@ -39,6 +39,17 @@ template <typename T>
 void launch_xattn_apply(const T* q, int ldq, const float* ctx, T* out, int ld_out, int n_scenes, int n_obj,
                         cudaStream_t s);
 void launch_xattn_prepare(const float* kv, int ld_kv, float* ctx, int n_scenes, int L, cudaStream_t s);
+// adjoints of the two (training step, backward.cu / pointwise.cu): dq (= | += by `accumulate`) and dctx
+// [n_scenes][4][32][32] fp32 from the kept pre-softmax q; dkv [n_scenes * L, 256] fp32 from kv and dctx
+template <typename T>
+void launch_xattn_apply_bwd(const T* q, int ldq, const T* dout, int ldo, const float* ctx, T* dq, int lddq,
+                            int accumulate, float* dctx, int n_scenes, int n_obj, cudaStream_t s);
+void launch_xattn_prepare_bwd(const float* kv, int ld_kv, const float* dctx, float* dkv, int ld_dkv, int n_scenes,
+                              int L, cudaStream_t s);
+// text tokens the prepare kernels hold in shared memory: 1 KB per token (k and v, 4 heads x 32 channels, fp32)
+// within the 200 KB dynamic shared-memory limit init_pointwise_attrs() raises them to
+constexpr int XATTN_SMEM_LIMIT = 200 * 1024;
+constexpr int XATTN_MAX_L = XATTN_SMEM_LIMIT / (4 * 2 * 32 * 4);
 
 void sinusoid_freqs_host(int dim, float* hf /*[dim / 2]*/);
 void launch_sinusoid(float* out, const float* freq_dev, int T, int dim, cudaStream_t s);

@@ -909,6 +909,72 @@ void launch_xattn_prepare(const float* kv, int ld_kv, float* ctx, int n_scenes, 
   k_xattn_prepare<<<n_scenes, 128, smem, s>>>(kv, ld_kv, ctx, n_scenes, L);
 }
 
+// adjoint of k_xattn_prepare (training step): dkv[scene * L + l][h * 32 + c] (k half) and [128 + h * 32 + c] (v half)
+// from dctx[scene][h][d][e].  k~ = softmax over the L tokens is recomputed; all arithmetic fp32.  Same shared memory
+// as k_xattn_prepare (k~ and v of the head, 1 KB per token for the CTA); v's slot is reused for dk~ once dv is out.
+//   dv[e][l] = sum_d dctx[d][e] k~[d][l]      dk~[d][l] = sum_e dctx[d][e] v[e][l]
+//   dk[d][l] = k~[d][l] (dk~[d][l] - sum_l' k~[d][l'] dk~[d][l'])
+__global__ void __launch_bounds__(128) k_xattn_prepare_bwd(const float* __restrict__ kv, int ld_kv,
+                                                           const float* __restrict__ dctx, float* __restrict__ dkv,
+                                                           int ld_dkv, int n_scenes, int L) {
+  extern __shared__ float sm[];
+  const int lane = threadIdx.x & 31, h = threadIdx.x >> 5;
+  const int scene = blockIdx.x;
+  float* ks = sm + h * 2 * L * 32;
+  float* vs = ks + L * 32;
+  const int64_t row0 = (int64_t)scene * L;
+  float kmax = -INFINITY;
+  for (int l = 0; l < L; ++l) {
+    const float* p = kv + (row0 + l) * ld_kv + h * 32 + lane;
+    float k = p[0];
+    ks[l * 32 + lane] = k;
+    vs[l * 32 + lane] = p[128];
+    kmax = fmaxf(kmax, k);
+  }
+  float ksum = 0.f;
+  for (int l = 0; l < L; ++l) {
+    float e = expf(ks[l * 32 + lane] - kmax);
+    ks[l * 32 + lane] = e;
+    ksum += e;
+  }
+  const float kinv = 1.0f / ksum;
+  for (int l = 0; l < L; ++l) ks[l * 32 + lane] *= kinv;
+  __syncwarp();
+  const float* dc = dctx + ((int64_t)scene * 4 + h) * 1024;
+  {      // lane = e: column e of dctx
+    float c[32];
+#pragma unroll
+    for (int d = 0; d < 32; ++d) c[d] = dc[d * 32 + lane];
+    for (int l = 0; l < L; ++l) {
+      float dv = 0.f;
+#pragma unroll
+      for (int d = 0; d < 32; ++d) dv = fmaf(c[d], ks[l * 32 + d], dv);
+      dkv[(row0 + l) * ld_dkv + 128 + h * 32 + lane] = dv;
+    }
+  }
+  {      // lane = d: row d of dctx
+    float r[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) r[e] = dc[lane * 32 + e];
+    float dot = 0.f;
+    for (int l = 0; l < L; ++l) {
+      float g = 0.f;
+#pragma unroll
+      for (int e = 0; e < 32; ++e) g = fmaf(r[e], vs[l * 32 + e], g);
+      __syncwarp();      // every lane has read v of token l before it is overwritten by dk~
+      vs[l * 32 + lane] = g;
+      dot = fmaf(ks[l * 32 + lane], g, dot);
+    }
+    for (int l = 0; l < L; ++l)
+      dkv[(row0 + l) * ld_dkv + h * 32 + lane] = ks[l * 32 + lane] * (vs[l * 32 + lane] - dot);
+  }
+}
+void launch_xattn_prepare_bwd(const float* kv, int ld_kv, const float* dctx, float* dkv, int ld_dkv, int n_scenes,
+                              int L, cudaStream_t s) {
+  size_t smem = size_t(4) * 2 * L * 32 * sizeof(float);
+  k_xattn_prepare_bwd<<<n_scenes, 128, smem, s>>>(kv, ld_kv, dctx, dkv, ld_dkv, n_scenes, L);
+}
+
 template <typename T>
 __global__ void __launch_bounds__(128) k_xattn_apply(const T* __restrict__ q, int ldq, const float* __restrict__ ctx,
                                                      T* __restrict__ out, int ld_out, int n_scenes, int n) {
@@ -1340,12 +1406,13 @@ void launch_loss_dict_mean(const float* parts, float* dict9, int B, cudaStream_t
 
 // raise the dynamic shared-memory limit of the attention cores once, outside any stream capture
 void init_pointwise_attrs() {
-  const int lim = 200 * 1024;
+  const int lim = XATTN_SMEM_LIMIT;
   cudaFuncSetAttribute(k_linattn<float, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
   cudaFuncSetAttribute(k_linattn<bf16, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
   cudaFuncSetAttribute(k_softattn<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
   cudaFuncSetAttribute(k_softattn<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
   cudaFuncSetAttribute(k_xattn_prepare, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
+  cudaFuncSetAttribute(k_xattn_prepare_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
 }
 
 // ---- explicit instantiations ----

@@ -134,6 +134,10 @@ struct TrainState {
         *dst = nullptr, *dtemb = nullptr, *dh1 = nullptr;
   float *ctx_act = nullptr, *ctx_film = nullptr, *dctx_film = nullptr, *dctx_act = nullptr;
   int ctx_rows_cap = 0;
+  // text cross-attention (fp32): per layer the text-side kv = cross W_kv^T [B*L, 256] and ctx [B, 4096], kept for the
+  // backward pass; one layer's dkv / dctx scratch (consumed right after that layer's adjoint)
+  float *xkv = nullptr, *xctx = nullptr, *dxkv = nullptr, *dxctx = nullptr;
+  int x_scenes_cap = 0, x_L_cap = 0;
   int* t_idx = nullptr;
   int* t_int = nullptr;
   float* x_t = nullptr;
@@ -169,7 +173,7 @@ void train_state_destroy(TrainState* t) {
   for (void* p : t->gbufs) cudaFree(p);
   cudaFree(t->warena); cudaFree(t->dwarena); cudaFree(t->varena); cudaFree(t->dvarena);
   for (float* p : {t->emb, t->z1, t->h1, t->temb, t->st, t->film, t->dfilm, t->dst, t->dtemb, t->dh1, t->ctx_act,
-                   t->ctx_film, t->dctx_film, t->dctx_act, t->x_t, t->loss_parts})
+                   t->ctx_film, t->dctx_film, t->dctx_act, t->x_t, t->loss_parts, t->xkv, t->xctx, t->dxkv, t->dxctx})
     cudaFree(p);
   cudaFree(t->t_idx); cudaFree(t->t_int);
   for (auto e : t->ev) if (e) cudaEventDestroy(e);
@@ -191,8 +195,6 @@ static int train_round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 static int train_init(ds_handle* h) {
   if (h->train) return 0;
-  if (h->cfg.text_condition)
-    return fail(DS_ERR_INVALID, "native training supports the unconditional / arrangement networks (no cross-attention backward)");
   TrainState* t = new TrainState();
   ds_config cfg = h->cfg;
   cfg.train = 1;
@@ -252,7 +254,7 @@ static int train_init(ds_handle* h) {
   return 0;
 }
 
-static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
+static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows, int cross_L) {
   TrainState* t = h->train;
   const Plan& P = t->plan;
   const int n_obj = h->cfg.num_objects, C = P.C;
@@ -430,6 +432,19 @@ static int train_capacity(ds_handle* h, int n_scenes, int ctx_rows) {
     CK(cudaMalloc(&t->dctx_film, (size_t)ctx_rows * ncb * 2 * C * 4));
     t->ctx_rows_cap = ctx_rows;
   }
+  if (cross_L > 0 && (n_scenes > t->x_scenes_cap || cross_L > t->x_L_cap)) {
+    const size_t nl = P.xattn_layers.size(), xs = std::max(n_scenes, t->x_scenes_cap), xl = std::max(cross_L, t->x_L_cap);
+    for (float** p : {&t->xkv, &t->xctx, &t->dxkv, &t->dxctx}) {
+      cudaFree(*p);
+      *p = nullptr;
+    }
+    CK(cudaMalloc(&t->xkv, nl * xs * xl * 256 * 4));
+    CK(cudaMalloc(&t->xctx, nl * xs * 4096 * 4));
+    CK(cudaMalloc(&t->dxkv, xs * xl * 256 * 4));
+    CK(cudaMalloc(&t->dxctx, xs * 4096 * 4));
+    t->x_scenes_cap = int(xs);
+    t->x_L_cap = int(xl);
+  }
   return 0;
 }
 
@@ -437,12 +452,13 @@ template <typename T>
 static int train_step_t(ds_handle* h, const float* flat, const float* x0, const int64_t* t64, const float* noise,
                         const float* context, int ctx_batch, int ctx_shared, int loss_separate, int loss_iou,
                         const float* bounds_host, float grad_scale, float* losses, float* loss_dict, float* grads,
-                        float* dcontext, int B, cudaStream_t s) {
+                        float* dcontext, const float* cross, int L, float* dcross, int B, cudaStream_t s) {
   TrainState* t = h->train;
   const Plan& P = t->plan;
   const ds_config& c = h->cfg;
   const int n_obj = c.num_objects, M = B * n_obj, C = P.C, E = c.cond_dim;
-  const int ntb = int(P.time_blocks.size()), ncb = int(P.ctx_blocks.size());
+  const int ntb = int(P.time_blocks.size()), ncb = int(P.ctx_blocks.size()), nxl = int(P.xattn_layers.size());
+  const int TD = c.text_dim;
   const int ctx_rows = ctx_shared ? n_obj : ctx_batch * n_obj;
   auto F = [&](const std::string& name) { return flat + t->flat_off.at(name); };
   auto G = [&](const std::string& name) { return grads + t->flat_off.at(name); };
@@ -514,6 +530,16 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
   for (int i = 0; i < ncb; ++i)
     f32gemm(t->ctx_act, E, E, F(P.ctx_blocks[i] + ".mlp.1.weight"), F(P.ctx_blocks[i] + ".mlp.1.bias"),
             t->ctx_film + (size_t)i * 2 * C, ncb * 2 * C, 2 * C, ctx_rows);
+  // text side of every LinearAttentionCross (denoise_net.py:284-293), as ds_set_context_cross computes it but from the
+  // flat parameters: kv = cross W_kv^T, ctx = softmax_L(k) v^T; both kept for the backward pass
+  auto xkv = [&](int l) { return t->xkv + (size_t)l * B * L * 256; };
+  auto xctx = [&](int l) { return t->xctx + (size_t)l * B * 4096; };
+  auto kv_name = [&](int l) { return P.xattn_layers[l] + ".fn.fn.to_kv.weight"; };
+  if (cross)
+    for (int l = 0; l < nxl; ++l) {
+      f32gemm(cross, TD, TD, F(kv_name(l)), nullptr, xkv(l), 256, 256, B * L);
+      launch_xattn_prepare(xkv(l), 256, xctx(l), B, L, s);
+    }
 
   auto film_of = [&](const Op& o) {
     FilmRef f;
@@ -566,6 +592,10 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
         break;
       case OP_ATTN:
         launch_softattn<T>(ptr(o.in0.buf, 0), ld(o.in0.buf), ptr(o.out, 0), ld(o.out), B, n_obj, s);
+        break;
+      case OP_XATTN:
+        if (!cross) return fail(DS_ERR_STATE, "op '%s' needs the text input", o.name.c_str());
+        launch_xattn_apply<T>(ptr(o.in0.buf, 0), ld(o.in0.buf), xctx(o.xlayer), ptr(o.out, 0), ld(o.out), B, n_obj, s);
         break;
       default:
         return fail(DS_ERR_STATE, "op kind %d has no training path", o.kind);
@@ -655,7 +685,7 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
     }
     return 0;
   };
-  bool dst_started = false, dctx_started = false;
+  bool dst_started = false, dctx_started = false, dcross_started = false;
   bool stT_ready = false;
   auto time_block_bwd = [&](int i) {      // FiLM projection of time block i: dW, db, and its share of d(SiLU(temb))
     const float* df = t->dfilm + (size_t)i * 2 * C;
@@ -785,6 +815,22 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
         launch_softattn_bwd<T>(ptr(o.in0.buf, 0), ld(o.in0.buf), gptr(o.out, 0), ld(o.out), gptr(o.in0.buf, 0), ld(o.in0.buf), B,
                                n_obj, s);
         break;
+      case OP_XATTN: {
+        // object side -> dq and dctx; text side -> dkv; then this layer's to_kv gradient and its share of d(cross), so
+        // that the to_kv weight is final (and its all-reduce bucket can go) as early as any other weight
+        const int qacc = first_write(o.in0.buf, 0);
+        launch_xattn_apply_bwd<T>(ptr(o.in0.buf, 0), ld(o.in0.buf), gptr(o.out, 0), ld(o.out), xctx(o.xlayer),
+                                  gptr(o.in0.buf, 0), ld(o.in0.buf), qacc, t->dxctx, B, n_obj, s);
+        launch_xattn_prepare_bwd(xkv(o.xlayer), 256, t->dxctx, t->dxkv, 256, B, L, s);
+        const std::string kn = kv_name(o.xlayer);
+        launch_gemm_tn<float, float>(t->dxkv, 256, cross, TD, G(kn), TD, B * L, 256, TD, s);
+        if (dcross) {
+          launch_gemm_nn<float, float, float>(t->dxkv, 256, F(kn), TD, dcross, TD, B * L, TD, 256, dcross_started ? 1 : 0, s);
+          dcross_started = true;
+        }
+        pending[kn] = false;
+        break;
+      }
       default:
         return fail(DS_ERR_STATE, "op kind %d has no backward", o.kind);
     }
@@ -827,12 +873,12 @@ extern "C" int64_t ds_train_param_count(ds_handle* h) {
   return n;
 }
 
-extern "C" int ds_train_step(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
-                             const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
-                             int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
-                             float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
-                             int32_t batch, void* stream) {
-  if (!h || !flat_params_dev || !x0_dev || !t_dev || !noise_dev || !context_dev || !losses_dev || !loss_dict_dev)
+static int train_step_impl(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
+                           const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
+                           int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
+                           float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
+                           const float* cross_dev, int32_t cross_L, float* dcross_dev, int32_t batch, void* stream) {
+  if (!flat_params_dev || !x0_dev || !t_dev || !noise_dev || !context_dev || !losses_dev || !loss_dict_dev)
     return fail(DS_ERR_INVALID, "null argument");
   if (h->T == 0) return fail(DS_ERR_STATE, "ds_set_schedule() has not been called");
   if (loss_iou && !bounds_host) return fail(DS_ERR_INVALID, "loss_iou needs bounds");
@@ -842,13 +888,46 @@ extern "C" int ds_train_step(ds_handle* h, const float* flat_params_dev, const f
   int rc = train_init(h);
   if (rc) return rc;
   const int ctx_rows = ctx_shared ? h->cfg.num_objects : ctx_batch * h->cfg.num_objects;
-  if ((rc = train_capacity(h, batch, ctx_rows))) return rc;
+  if ((rc = train_capacity(h, batch, ctx_rows, cross_dev ? cross_L : 0))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (h->train->bf16)
     return train_step_t<bf16>(h, flat_params_dev, x0_dev, t_dev, noise_dev, context_dev, ctx_batch, ctx_shared, loss_separate,
-                              loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev, batch, s);
+                              loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev,
+                              cross_dev, cross_L, dcross_dev, batch, s);
   return train_step_t<float>(h, flat_params_dev, x0_dev, t_dev, noise_dev, context_dev, ctx_batch, ctx_shared, loss_separate,
-                             loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev, batch, s);
+                             loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev,
+                             cross_dev, cross_L, dcross_dev, batch, s);
+}
+
+static_assert(XATTN_MAX_L == DS_TRAIN_CROSS_MAX_L, "the header's text-length limit must match the prepare kernels");
+
+extern "C" int ds_train_step(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
+                             const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
+                             int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
+                             float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
+                             int32_t batch, void* stream) {
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  if (h->cfg.text_condition)
+    return fail(DS_ERR_INVALID, "this network has text cross-attention: train it with ds_train_step_cross (text input)");
+  return train_step_impl(h, flat_params_dev, x0_dev, t_dev, noise_dev, context_dev, ctx_batch, ctx_shared, loss_separate,
+                         loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev,
+                         nullptr, 0, nullptr, batch, stream);
+}
+
+extern "C" int ds_train_step_cross(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
+                                   const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
+                                   int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
+                                   float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
+                                   const float* cross_dev, int32_t cross_L, float* dcross_dev, int32_t batch, void* stream) {
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  if (!h->cfg.text_condition)
+    return fail(DS_ERR_INVALID, "configuration has no text condition: train it with ds_train_step");
+  if (!cross_dev) return fail(DS_ERR_INVALID, "a text-conditioned network needs cross_dev [batch, L, text_dim]");
+  if (cross_L < 1 || cross_L > DS_TRAIN_CROSS_MAX_L)
+    return fail(DS_ERR_INVALID, "text length %d outside [1, %d]", cross_L, DS_TRAIN_CROSS_MAX_L);
+  return train_step_impl(h, flat_params_dev, x0_dev, t_dev, noise_dev, context_dev, ctx_batch, ctx_shared, loss_separate,
+                         loss_iou, bounds_host, grad_scale, losses_dev, loss_dict_dev, flat_grads_dev, dcontext_dev,
+                         cross_dev, cross_L, dcross_dev, batch, stream);
 }
 
 extern "C" int ds_train_set_buckets(ds_handle* h, const int64_t* bounds, int32_t n_buckets, void* const* events) {

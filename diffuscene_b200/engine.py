@@ -239,9 +239,12 @@ class DenoiserEngine:
     def train_step(self, flat_params: torch.Tensor, x0: torch.Tensor, t: torch.Tensor, noise: torch.Tensor,
                    context: torch.Tensor, shared: bool, loss_separate: bool, loss_iou: bool,
                    bounds: Optional[Sequence[float]] = None, flat_grads: Optional[torch.Tensor] = None,
-                   want_dcontext: bool = True, grad_scale: float = 1.0):
+                   want_dcontext: bool = True, grad_scale: float = 1.0, cross: Optional[torch.Tensor] = None,
+                   want_dcross: bool = True):
         """Forward of p_losses + the native backward pass: (losses [B], loss dict, d(context) or None).
-        Gradients of every denoiser parameter land in `flat_grads` (flat_layout order)."""
+        Gradients of every denoiser parameter land in `flat_grads` (flat_layout order).
+        Text-conditioned networks pass `cross` (context_cross [B, L, text_dim]); the result then has a fourth entry,
+        d(cross) or None (ds_train_step_cross)."""
         assert flat_params.is_cuda and flat_params.dtype == torch.float32 and flat_params.is_contiguous()
         x0, t, noise = x0.contiguous(), t.to(self.device).contiguous(), noise.contiguous()
         ctx = context.detach().to(self.device, torch.float32).contiguous()
@@ -250,11 +253,16 @@ class DenoiserEngine:
         ld = torch.empty(9, device=self.device, dtype=torch.float32)
         dctx = torch.empty_like(ctx) if (want_dcontext and flat_grads is not None) else None
         barr = None if bounds is None else (C.c_float * 12)(*[float(v) for v in bounds])
-        capi.check(self.lib.ds_train_step(self.h, _ptr(flat_params), _ptr(x0), _ptr(t), _ptr(noise), _ptr(ctx),
-                                          0 if shared else B, int(bool(shared)), int(loss_separate), int(loss_iou), barr,
-                                          float(grad_scale), _ptr(losses), _ptr(ld), _ptr(flat_grads), _ptr(dctx), B,
-                                          self._stream()))
-        return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}, dctx
+        args = (self.h, _ptr(flat_params), _ptr(x0), _ptr(t), _ptr(noise), _ptr(ctx), 0 if shared else B,
+                int(bool(shared)), int(loss_separate), int(loss_iou), barr, float(grad_scale), _ptr(losses), _ptr(ld),
+                _ptr(flat_grads), _ptr(dctx))
+        if cross is None:
+            capi.check(self.lib.ds_train_step(*args, B, self._stream()))
+            return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}, dctx
+        xc = cross.detach().to(self.device, torch.float32).contiguous()
+        dxc = torch.empty_like(xc) if (want_dcross and flat_grads is not None) else None
+        capi.check(self.lib.ds_train_step_cross(*args, _ptr(xc), xc.shape[1], _ptr(dxc), B, self._stream()))
+        return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}, dctx, dxc
 
     def train_set_buckets(self, bounds: Sequence[int], events: Sequence["torch.cuda.Event"]):
         """Gradient buckets for the overlapped all-reduce (see ds_train_set_buckets); `events` are torch.cuda.Event

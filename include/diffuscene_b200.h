@@ -184,19 +184,35 @@ DS_API int ds_p_losses(ds_handle* h, const float* x0_dev, const int64_t* t_dev, 
  * (scene_synthesis/networks/diffusion_scene_layout_ddpm.py:456-473) for the denoiser: forward of p_losses
  * (diffusion_ddpm.py:520-652) with every intermediate kept, then the hand-written backward pass of every layer of
  * Unet1D (denoise_net.py:78-593: weight-standardised convs, GroupNorm + FiLM + SiLU blocks, LayerNorms, linear /
- * softmax attention, the time-embedding MLP and all FiLM projections) and of the loss (MSE terms + IoU regulariser).
+ * softmax attention, text cross-attention, the time-embedding MLP and all FiLM projections) and of the loss (MSE terms
+ * + IoU regulariser).
  * Parameters and gradients are ONE flat fp32 device buffer each, laid out in ds_expected_weight() order
  * (ds_train_param_count() floats).  grad_scale multiplies d(mean-over-batch loss); pass 1 / world_size to get the
  * data-parallel mean after a sum all-reduce.  context [ctx_shared ? N : B*N, cond_dim] is the conditioning input of
  * Unet1D.forward; dcontext_dev (optional, same shape) receives its gradient (it continues into
  * positional_embedding / the condition MLPs on the caller's side).  flat_grads_dev == NULL: forward + loss only.
- * Uses the handle's schedule (ds_set_schedule) and precision; networks with text cross-attention are not supported. */
+ * Uses the handle's schedule (ds_set_schedule) and precision.  Networks with text cross-attention
+ * (text_condition != 0) train through ds_train_step_cross; ds_train_step returns DS_ERR_INVALID for them. */
 DS_API int64_t ds_train_param_count(ds_handle* h);
 DS_API int ds_train_step(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
                          const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
                          int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
                          float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
                          int32_t batch, void* stream);
+/* Longest text ds_train_step_cross accepts: the text-side kernels keep k and v of every token in shared memory,
+ * 1 KB per token within a 200 KB limit.  BERT descriptions of the reference are far shorter. */
+#define DS_TRAIN_CROSS_MAX_L 200
+/* ds_train_step for the text-conditioned networks (LinearAttentionCross layers, denoise_net.py:261-297): the same
+ * arguments, plus cross_dev = context_cross [batch, cross_L, text_dim] fp32 on the device (the projected text, as in
+ * ds_set_context_cross).  The gradients of every to_kv weight land in flat_grads_dev like all others; dcross_dev
+ * (optional, same shape as cross_dev, overwritten) receives d(loss)/d(cross), which continues into the text
+ * projection (fc_text_f) on the caller's side.  DS_ERR_INVALID for a network without text condition, a NULL cross_dev
+ * or cross_L outside [1, DS_TRAIN_CROSS_MAX_L]. */
+DS_API int ds_train_step_cross(ds_handle* h, const float* flat_params_dev, const float* x0_dev, const int64_t* t_dev,
+                               const float* noise_dev, const float* context_dev, int32_t ctx_batch, int32_t ctx_shared,
+                               int32_t loss_separate, int32_t loss_iou, const float* bounds_host, float grad_scale,
+                               float* losses_dev, float* loss_dict_dev, float* flat_grads_dev, float* dcontext_dev,
+                               const float* cross_dev, int32_t cross_L, float* dcross_dev, int32_t batch, void* stream);
 /* Overlap of the data-parallel gradient all-reduce with the backward pass: bucket k is the flat range
  * [bounds[k], bounds[k + 1]) (bounds[0] = 0, bounds[n] = ds_train_param_count()); ds_train_step records events[k] (a
  * cudaEvent_t owned by the caller) on its stream as soon as every gradient inside the bucket is final -- the backward
