@@ -11,7 +11,8 @@
 //   wgmma       warpgroup g multiplies rows 64 g .. 64 g + 63 of the A tile with the whole W tile:
 //               wgmma.mma_async m64n128k16 x 4 per k-block, accumulator in 64 registers per thread.
 //               Two resident CTAs per SM let one CTA's epilogue overlap the other's MMAs.
-//   epilogue    straight from the accumulator registers.  Three forms:
+//   epilogue    from the accumulator registers; bf16 results are staged in the drained ring and written out as
+//               whole 256-byte rows.  Three forms:
 //                 plain  bias / GELU|SiLU / residual -> bf16
 //                 d32    split-K partial sums added to an fp32 output with atomics (weight-gradient GEMMs)
 //                 GN     the whole `Block` of the reference (denoise_net.py:160-176) after the conv:
@@ -43,6 +44,10 @@ static constexpr int PART_OFF = CHAN_OFF + 3 * BN * 4;
 static constexpr int STAT_OFF = PART_OFF + BM * 2 * 8;
 static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAT_OFF + BM * 2 * 8;
 static_assert(2 * (SMEM_BYTES + 1024) <= 233472, "two CTAs per SM");
+// bf16 output tile staged in the drained ring before it is written out; the row pitch of 136 elements (68 words) puts
+// the 8 rows one fragment store touches on distinct banks
+static constexpr int STG_PITCH = BN + 8;
+static_assert(BM * STG_PITCH * 2 <= STAGES * STAGE_BYTES, "staging tile fits in the ring");
 
 struct TcEpi {
   const float* bias;
@@ -207,13 +212,16 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
       stat[tid] = make_float2(mean, rsqrtf(var + 1e-5f));
     }
     __syncthreads();
+  } else {
+    __syncthreads();        // the other warpgroup's MMAs may still read the ring the tile is staged in
   }
 
+  bf16* const stg = reinterpret_cast<bf16*>(base_ptr);      // [BM][STG_PITCH]
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int rt = r0 + 8 * h, m = m0 + rt;
     if (rt >= epi.tile_rows || m >= epi.M) continue;
-    bf16* dp = epi.d + (int64_t)m * epi.ldd + n0 + cq;
+    bf16* sp = stg + rt * STG_PITCH + cq;
     const bf16* rp = epi.res ? epi.res + (int64_t)m * epi.ldres + n0 + cq : nullptr;
     int sc = 0;
     const float* frow = nullptr;         // FiLM row of this token: [scale(C) | shift(C)], already at column n0
@@ -254,8 +262,17 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
         v[0] += r2.x;
         v[1] += r2.y;
       }
-      *reinterpret_cast<__nv_bfloat162*>(dp + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
+      *reinterpret_cast<__nv_bfloat162*>(sp + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
     }
+  }
+  __syncthreads();
+  // whole output rows: 16 threads x 16 bytes per 256-byte row, instead of the fragment layout's 16 bytes per row and
+  // store instruction
+  for (int idx = tid; idx < BM * (BN / 8); idx += TC_THREADS) {
+    const int rt = idx / (BN / 8), c = (idx % (BN / 8)) * 8, m = m0 + rt;
+    if (rt < epi.tile_rows && m < epi.M)
+      *reinterpret_cast<uint4*>(epi.d + (int64_t)m * epi.ldd + n0 + c) =
+          *reinterpret_cast<const uint4*>(stg + rt * STG_PITCH + c);
   }
 }
 
