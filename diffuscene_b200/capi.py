@@ -41,6 +41,13 @@ class DsSampleArgs(C.Structure):
         ("chunk_scenes", C.c_int32), ("reserved", C.c_int32 * 5)]
 
 
+class DsVlbArgs(C.Structure):
+    _fields_ = [
+        ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
+        ("scene_offset", C.c_uint64), ("noise_dev", C.c_void_p), ("use_graph", C.c_int32),
+        ("reserved", C.c_int32 * 7)]
+
+
 _lib = None
 
 
@@ -67,6 +74,8 @@ def load(rebuild: bool = False):
         "ds_expected_weight_count": (C.c_int, [H]),
         "ds_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
         "ds_set_schedule": (C.c_int, [H, C.POINTER(DsSchedule)]),
+        "ds_set_vlb_schedule": (C.c_int, [H, C.c_int32, p, p, p]),
+        "ds_vlb_loop": (C.c_int, [H, C.POINTER(DsVlbArgs), p, p, p, p]),
         "ds_set_context": (C.c_int, [H, p, C.c_int32, C.c_int32, p]),
         "ds_set_context_cross": (C.c_int, [H, p, C.c_int32, C.c_int32, p]),
         "ds_denoise_forward": (C.c_int, [H, p, p, p, C.c_int32, p]),
@@ -106,7 +115,8 @@ def load(rebuild: bool = False):
 
 
 EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_weight", "ds_commit_weights",
-            "ds_expected_weight_count", "ds_expected_weight", "ds_set_schedule", "ds_set_context",
+            "ds_expected_weight_count", "ds_expected_weight", "ds_set_schedule", "ds_set_vlb_schedule", "ds_vlb_loop",
+            "ds_set_context",
             "ds_set_context_cross", "ds_denoise_forward", "ds_denoise_forward_host", "ds_sample_loop",
             "ds_sample_loop_host", "ds_traj_count", "ds_p_sample_step", "ds_q_sample", "ds_p_losses", "ds_retrieve_objects",
             "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_sumsq", "ds_adam_step",

@@ -28,6 +28,9 @@ void drop_graph(ds_handle* h) {
   if (h->gexec) cudaGraphExecDestroy(h->gexec);
   h->gexec = nullptr;
   h->gkey = ds_handle::GraphKey();
+  if (h->vexec) cudaGraphExecDestroy(h->vexec);
+  h->vexec = nullptr;
+  h->vkey = ds_handle::VlbKey();
   h->plan_gen++;
 }
 
@@ -518,6 +521,7 @@ extern "C" int ds_destroy(ds_handle* h) {
   cudaFree(h->xctx);
   for (int i = 0; i < S_COUNT; ++i) cudaFree(h->sched_dev[i]);
   cudaFree(h->coef_dev); cudaFree(h->state_dev);
+  cudaFree(h->vlb_coef); cudaFree(h->vlb_x0); cudaFree(h->vlb_vb); cudaFree(h->vlb_mse);
   if (h->own_stream) cudaStreamDestroy(h->own_stream);
   delete h;
   return 0;
@@ -566,12 +570,28 @@ extern "C" int ds_set_schedule(ds_handle* h, const ds_schedule* s) {
     h->sched_host[S_NEG_1MAC][t] = -s->sqrt_1mac[t];
     h->sched_host[S_NEG_RECIPM1][t] = -s->sqrt_recipm1_ac[t];
   }
-  for (int i = 0; i < S_COUNT; ++i) {
+  for (int i = 0; i < S_VLB_FIRST; ++i) {
     int rc = upload_f32(&h->sched_dev[i], h->sched_host[i].data(), s->T);
     if (rc) return rc;
   }
   h->T = s->T;
   h->mean_type = s->mean_type;
+  return 0;
+}
+
+extern "C" int ds_set_vlb_schedule(ds_handle* h, int32_t T, const float* post_logvar, const float* model_logvar,
+                                   const float* log_1mac) {
+  if (!h || !post_logvar || !model_logvar || !log_1mac) return fail(DS_ERR_INVALID, "null argument");
+  if (T != h->cfg.num_timesteps)
+    return fail(DS_ERR_INVALID, "VLB tables have T=%d, the configured num_timesteps is %d", T, h->cfg.num_timesteps);
+  CK(cudaSetDevice(h->cfg.device));
+  const float* src[3] = {post_logvar, model_logvar, log_1mac};
+  for (int i = 0; i < 3; ++i) {
+    h->sched_host[S_VLB_FIRST + i].assign(src[i], src[i] + T);
+    int rc = upload_f32(&h->sched_dev[S_VLB_FIRST + i], src[i], T);
+    if (rc) return rc;
+  }
+  h->vlb_set = true;
   return 0;
 }
 
@@ -895,6 +915,121 @@ extern "C" int ds_sample_loop_host(ds_handle* h, const ds_sample_args* a, float*
   if ((rc = ds_sample_loop(h, a, h->x_tmp, h->own_stream))) return rc;
   CK(cudaMemcpyAsync(out_host, h->x_tmp, xs, cudaMemcpyDeviceToHost, h->own_stream));
   CK(cudaStreamSynchronize(h->own_stream));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// variational bound (calc_bpd_loop, diffusion_ddpm.py:690-717)
+// ------------------------------------------------------------------------------------------------
+// one loop iteration: x_t = q_sample(x0, t) (k_begin_step with every object "partial") -> denoiser -> VLB terms at t
+static int vlb_body(ds_handle* h, const ds_vlb_args* a, cudaStream_t s) {
+  const Plan& P = h->plan;
+  const int B = a->batch, n_obj = h->cfg.num_objects;
+  launch_begin_step(h->vlb_coef, h->state_dev, h->t_dev, h->x_state, h->vlb_x0, a->noise_dev, B, n_obj, P.d, n_obj, s);
+  h->launches++;
+  int rc = run_forward(h, h->x_state, B, s);
+  if (rc) return rc;
+  const float *lv1 = h->sched_dev[S_POST_LOGVAR], *lv2 = h->sched_dev[S_MODEL_LOGVAR];
+  if (h->bf16_mode)
+    launch_vlb_terms<bf16>(h->vlb_coef, h->state_dev, h->x_state, (const bf16*)h->bufs[P.out_buf], P.dpad, h->vlb_x0,
+                           lv1, lv2, h->vlb_vb, h->vlb_mse, B, n_obj, P.d, h->T, a->clip_denoised, s);
+  else
+    launch_vlb_terms<float>(h->vlb_coef, h->state_dev, h->x_state, (const float*)h->bufs[P.out_buf], P.dpad,
+                            h->vlb_x0, lv1, lv2, h->vlb_vb, h->vlb_mse, B, n_obj, P.d, h->T, a->clip_denoised, s);
+  h->launches++;
+  return 0;
+}
+
+extern "C" int ds_vlb_loop(ds_handle* h, const ds_vlb_args* a, float* vb_dev, float* mse_dev, float* prior_dev,
+                           void* stream) {
+  if (!h || !a || !a->x0_dev || !prior_dev) return fail(DS_ERR_INVALID, "null argument");
+  if ((vb_dev == nullptr) != (mse_dev == nullptr))
+    return fail(DS_ERR_INVALID, "vb_dev and mse_dev are both given or both NULL");
+  if (a->batch <= 0) return fail(DS_ERR_INVALID, "batch must be positive");
+  if (h->T == 0) return fail(DS_ERR_STATE, "ds_set_schedule() has not been called");
+  if (!h->vlb_set) return fail(DS_ERR_STATE, "ds_set_vlb_schedule() has not been called");
+  CK(cudaSetDevice(h->cfg.device));
+  const Plan& P = h->plan;
+  const int B = a->batch, n_obj = h->cfg.num_objects, T = h->T;
+  const int per_scene = n_obj * P.d;
+  cudaStream_t s = stream ? (cudaStream_t)stream : h->own_stream;
+  int rc = 0;
+  if (vb_dev) {
+    if ((rc = ensure_capacity(h, B))) return rc;
+    if ((rc = check_ready(h, B))) return rc;
+    if (B > h->vlb_cap) {
+      cudaFree(h->vlb_x0); cudaFree(h->vlb_vb); cudaFree(h->vlb_mse);
+      h->vlb_x0 = h->vlb_vb = h->vlb_mse = nullptr;
+      h->vlb_cap = 0;
+      CK(cudaMalloc(&h->vlb_x0, sizeof(float) * B * per_scene));
+      CK(cudaMalloc(&h->vlb_vb, sizeof(float) * B * T));
+      CK(cudaMalloc(&h->vlb_mse, sizeof(float) * B * T));
+      h->vlb_cap = B;
+    }
+    if (!h->vlb_coef) CK(cudaMalloc(&h->vlb_coef, sizeof(StepCoef) * T));
+    // loop order t = T-1 .. 0 (:696); the c_z column is unused
+    std::vector<StepCoef> coef(T);
+    for (int i = 0; i < T; ++i) {
+      const int t = T - 1 - i;
+      StepCoef& c = coef[i];
+      model_coefs(h, t, &c.a_x, &c.a_o);
+      c.c_0 = h->sched_host[S_COEF1][t];
+      c.c_x = h->sched_host[S_COEF2][t];
+      c.c_z = 0.f;
+      c.q_a = h->sched_host[S_SQRT_AC][t];
+      c.q_b = h->sched_host[S_SQRT_1MAC][t];
+      c.t = t;
+    }
+    CK(cudaMemcpyAsync(h->vlb_coef, coef.data(), sizeof(StepCoef) * T, cudaMemcpyHostToDevice, s));
+    StepState st0;
+    st0.step = 0; st0.done = 0; st0.seed = a->seed; st0.scene_offset = a->scene_offset;
+    CK(cudaMemcpyAsync(h->state_dev, &st0, sizeof(StepState), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->vlb_x0, a->x0_dev, sizeof(float) * B * per_scene, cudaMemcpyDeviceToDevice, s));
+    CK(cudaStreamSynchronize(s));      // coef / st0 are locals
+
+    cudaGraphExec_t vexec = nullptr;
+    int64_t launches_per_step = 0;
+    if (a->use_graph) {
+      ds_handle::VlbKey key;
+      key.batch = B; key.clip = a->clip_denoised; key.plan_gen = h->plan_gen; key.noise = a->noise_dev;
+      key.x0 = h->vlb_x0; key.vb = h->vlb_vb; key.mse = h->vlb_mse; key.coef = h->vlb_coef;
+      key.lv1 = h->sched_dev[S_POST_LOGVAR]; key.lv2 = h->sched_dev[S_MODEL_LOGVAR]; key.stream = s;
+      if (!h->vexec || !(h->vkey == key)) {
+        if (h->vexec) { cudaGraphExecDestroy(h->vexec); h->vexec = nullptr; }
+        cudaGraph_t graph = nullptr;
+        int64_t l0 = h->launches;
+        CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+        rc = vlb_body(h, a, s);
+        cudaError_t ce = cudaStreamEndCapture(s, &graph);
+        if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+        if (ce != cudaSuccess) return fail(DS_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(ce));
+        ce = cudaGraphInstantiate(&h->vexec, graph, 0);
+        cudaGraphDestroy(graph);
+        if (ce != cudaSuccess) { h->vexec = nullptr; return fail(DS_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(ce)); }
+        h->v_launches = h->launches - l0;
+        h->launches = l0;
+        h->vkey = key;
+      }
+      vexec = h->vexec;
+      launches_per_step = h->v_launches;
+    }
+    for (int i = 0; i < T; ++i) {
+      if (vexec) {
+        CK(cudaGraphLaunch(vexec, s));
+        h->launches += launches_per_step;
+      } else if ((rc = vlb_body(h, a, s))) {
+        return rc;
+      }
+    }
+    CK(cudaMemcpyAsync(vb_dev, h->vlb_vb, sizeof(float) * B * T, cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(mse_dev, h->vlb_mse, sizeof(float) * B * T, cudaMemcpyDeviceToDevice, s));
+  }
+  launch_prior_bpd(a->x0_dev, h->sched_dev[S_SQRT_AC], h->sched_dev[S_LOG_1MAC], T - 1, B, per_scene, prior_dev, s);
+  h->launches++;
+  cudaError_t le = cudaGetLastError();
+  if (vb_dev || !stream) CK(cudaStreamSynchronize(s));      // the caller's injected noise may go away after the call
+  if (le != cudaSuccess) return fail(DS_ERR_CUDA, "VLB loop: %s", cudaGetErrorString(le));
+  if (tc_error_flag()) return fail(DS_ERR_CUDA, "tensor-core GEMM pipeline timeout (code %d)", tc_error_flag());
   return 0;
 }
 

@@ -28,8 +28,10 @@ int fail(int code, const char* fmt, ...);      // engine.cu: records the message
       return fail(DS_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
   } while (0)
 
+// S_POST_LOGVAR .. S_LOG_1MAC are the variational-bound tables of ds_set_vlb_schedule; ds_set_schedule fills the rest
 enum { S_SQRT_AC = 0, S_SQRT_1MAC, S_SQRT_RECIP, S_SQRT_RECIPM1, S_COEF1, S_COEF2, S_SIGMA, S_AC, S_LW, S_NEG_1MAC,
-       S_NEG_RECIPM1, S_ZERO, S_ONE, S_COUNT };
+       S_NEG_RECIPM1, S_ZERO, S_ONE, S_POST_LOGVAR, S_MODEL_LOGVAR, S_LOG_1MAC, S_COUNT };
+constexpr int S_VLB_FIRST = S_POST_LOGVAR;
 
 struct TrainState;
 void train_state_destroy(TrainState* t);      // train.cu
@@ -92,6 +94,25 @@ struct ds_handle {
   int64_t g_launches = 0;     // kernel launches inside one replay
   int plan_gen = 0;           // bumped whenever buffers / tensor maps / tables are rebuilt
   int64_t graph_builds = 0;
+  // variational bound (ds_vlb_loop): its own step graph, coefficient table and staging buffers, so that a VLB call
+  // neither evicts nor rebuilds the sampling graph above.  The key holds every pointer the capture bakes in that
+  // plan_gen does not cover.
+  bool vlb_set = false;                 // ds_set_vlb_schedule() has been called
+  struct VlbKey {
+    int batch = -1, clip = 0, plan_gen = 0;
+    const void *noise = nullptr, *x0 = nullptr, *vb = nullptr, *mse = nullptr, *coef = nullptr, *lv1 = nullptr,
+               *lv2 = nullptr;
+    cudaStream_t stream = nullptr;
+    bool operator==(const VlbKey& o) const {
+      return batch == o.batch && clip == o.clip && plan_gen == o.plan_gen && noise == o.noise && x0 == o.x0 &&
+             vb == o.vb && mse == o.mse && coef == o.coef && lv1 == o.lv1 && lv2 == o.lv2 && stream == o.stream;
+    }
+  } vkey;
+  cudaGraphExec_t vexec = nullptr;
+  int64_t v_launches = 0;
+  StepCoef* vlb_coef = nullptr;         // [T] per-step coefficients of the VLB loop (step i <-> t = T-1-i)
+  float *vlb_x0 = nullptr, *vlb_vb = nullptr, *vlb_mse = nullptr;      // [cap, N, d], [cap, T], [cap, T]
+  int vlb_cap = 0;
   TrainState* train = nullptr;      // lazily created by ds_train_* (train.cu)
 };
 void drop_graph(ds_handle* h);

@@ -90,6 +90,19 @@ void launch_p_sample(const float* x, const T* model_out, int ld_out, const int* 
 void launch_q_sample(const float* x0, const int64_t* t, const float* noise, float* out, const float* sqrt_ac,
                      const float* sqrt_1mac, int B, int per_scene, cudaStream_t s);
 
+// variational bound (diffusion_ddpm.py:511-518, 679-717), one CTA per scene, fixed-order reductions (no atomics).
+// End of a VLB step: x = x_t of the step (k_begin_step with P = n_obj, partial = x0), coef[step] holds the x0
+// conversion (a_x, a_o), the posterior-mean coefficients (c_0, c_x) and t.  vb[b][t] = mean KL(true posterior ||
+// model) / ln 2 with logvar1 = post_logvar[t], logvar2 = model_logvar[t]; mse[b][t] = mean (x0_hat - x0)^2.
+// Advances st->step.
+template <typename T>
+void launch_vlb_terms(const StepCoef* coef, StepState* st, const float* x, const T* model_out, int ld_out,
+                      const float* x0, const float* post_logvar, const float* model_logvar, float* vb /*[B][n_t]*/,
+                      float* mse /*[B][n_t]*/, int B, int n_obj, int d, int n_t, int clip, cudaStream_t s);
+// prior[b] = mean KL(N(sqrt_ac[t_last] x0, exp(log_1mac[t_last])) || N(0, 1)) / ln 2
+void launch_prior_bpd(const float* x0, const float* sqrt_ac, const float* log_1mac, int t_last, int B, int per_scene,
+                      float* prior, cudaStream_t s);
+
 // p_losses value (reference diffusion_ddpm.py:520-652): one CTA per scene
 struct LossArgs {
   int n_obj, d, trans, size, angle, cls, objn, feat;

@@ -1238,6 +1238,101 @@ void launch_q_sample(const float* x0, const int64_t* t, const float* noise, floa
 }
 
 // ------------------------------------------------------------------------------------------------
+// variational bound (diffusion_ddpm.py:96-101, 511-518, 679-717): one CTA (128 threads) per scene
+// ------------------------------------------------------------------------------------------------
+// the per-element part of normal_kl: 0.5 * (a + (m1 - m2)^2 * e) with a = ((-1 + lv2) - lv1) + exp(lv1 - lv2) and
+// e = exp(-lv2), evaluated left to right like the reference's torch expression, every product / sum rounded
+__device__ __forceinline__ float kl_elem(float a, float e, float m1, float m2) {
+  const float dm = __fsub_rn(m1, m2);
+  return __fmul_rn(0.5f, __fadd_rn(a, __fmul_rn(__fmul_rn(dm, dm), e)));
+}
+__device__ __forceinline__ float kl_const(float lv1, float lv2) {
+  return __fadd_rn(__fsub_rn(__fadd_rn(-1.0f, lv2), lv1), expf(__fsub_rn(lv1, lv2)));
+}
+// sum over the CTA in a fixed order: per-thread serial sums, the warp butterfly, then warps 0..3 in order
+__device__ __forceinline__ float cta128_sum(float v, float* red) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  const float r = __fadd_rn(__fadd_rn(__fadd_rn(red[0], red[1]), red[2]), red[3]);
+  __syncthreads();
+  return r;
+}
+
+constexpr float kLn2 = 0.693147180559945309f;
+
+// KL(q(x_{t-1} | x_t, x0) || p(x_{t-1} | x_t)) and the x0-prediction MSE of every scene at the step's t; x = x_t
+// (written by k_begin_step), model_out the denoiser output at (x_t, t).  vb / mse are [B][n_t] (row = scene).
+template <typename T>
+__global__ void __launch_bounds__(128) k_vlb_terms(const StepCoef* __restrict__ coef, StepState* st,
+                                                   const float* __restrict__ x, const T* __restrict__ model_out,
+                                                   int ld_out, const float* __restrict__ x0,
+                                                   const float* __restrict__ post_logvar,
+                                                   const float* __restrict__ model_logvar, float* __restrict__ vb,
+                                                   float* __restrict__ mse, int n_obj, int d, int n_t, int clip) {
+  __shared__ float red[4];
+  const int step = st->step;
+  const StepCoef c = coef[step];
+  const int b = blockIdx.x, per_scene = n_obj * d;
+  const float lv2 = model_logvar[c.t];
+  const float a = kl_const(post_logvar[c.t], lv2), e = expf(-lv2);
+  float s_kl = 0.f, s_se = 0.f;
+  for (int i = threadIdx.x; i < per_scene; i += 128) {
+    const int o = i / d, ch = i % d;
+    const int64_t xi = (int64_t)b * per_scene + i;
+    const float xv = x[xi], x0v = x0[xi];
+    const float ov = ldf(model_out + ((int64_t)b * n_obj + o) * ld_out + ch);
+    float xh = __fadd_rn(__fmul_rn(c.a_x, xv), __fmul_rn(c.a_o, ov));
+    if (clip) xh = fminf(fmaxf(xh, -1.0f), 1.0f);
+    const float m_true = __fadd_rn(__fmul_rn(c.c_0, x0v), __fmul_rn(c.c_x, xv));
+    const float m_model = __fadd_rn(__fmul_rn(c.c_0, xh), __fmul_rn(c.c_x, xv));
+    s_kl = __fadd_rn(s_kl, kl_elem(a, e, m_true, m_model));
+    const float df = __fsub_rn(xh, x0v);
+    s_se = __fadd_rn(s_se, __fmul_rn(df, df));
+  }
+  const float kl = cta128_sum(s_kl, red), se = cta128_sum(s_se, red);
+  if (threadIdx.x == 0) {
+    const float n = float(per_scene);
+    vb[(int64_t)b * n_t + c.t] = __fdiv_rn(__fdiv_rn(kl, n), kLn2);
+    mse[(int64_t)b * n_t + c.t] = __fdiv_rn(se, n);
+    // the last block to finish advances the loop counter (every block has read st->step by then)
+    __threadfence();
+    unsigned int done = atomicAdd(&st->done, 1u);
+    if (done == gridDim.x - 1) {
+      st->done = 0;
+      st->step = step + 1;
+      __threadfence();
+    }
+  }
+}
+template <typename T>
+void launch_vlb_terms(const StepCoef* coef, StepState* st, const float* x, const T* model_out, int ld_out,
+                      const float* x0, const float* post_logvar, const float* model_logvar, float* vb, float* mse,
+                      int B, int n_obj, int d, int n_t, int clip, cudaStream_t s) {
+  k_vlb_terms<T><<<B, 128, 0, s>>>(coef, st, x, model_out, ld_out, x0, post_logvar, model_logvar, vb, mse, n_obj, d,
+                                   n_t, clip);
+}
+
+// _prior_bpd: KL(q(x_{T-1} | x0) || N(0, 1)) per scene, in bits per dimension
+__global__ void __launch_bounds__(128) k_prior_bpd(const float* __restrict__ x0, const float* __restrict__ sqrt_ac,
+                                                   const float* __restrict__ log_1mac, int t_last, int per_scene,
+                                                   float* __restrict__ prior) {
+  __shared__ float red[4];
+  const int b = blockIdx.x;
+  const float sa = sqrt_ac[t_last];
+  const float a = kl_const(log_1mac[t_last], 0.0f);
+  float s_kl = 0.f;
+  for (int i = threadIdx.x; i < per_scene; i += 128)
+    s_kl = __fadd_rn(s_kl, kl_elem(a, 1.0f, __fmul_rn(sa, x0[(int64_t)b * per_scene + i]), 0.0f));
+  const float kl = cta128_sum(s_kl, red);
+  if (threadIdx.x == 0) prior[b] = __fdiv_rn(__fdiv_rn(kl, float(per_scene)), kLn2);
+}
+void launch_prior_bpd(const float* x0, const float* sqrt_ac, const float* log_1mac, int t_last, int B, int per_scene,
+                      float* prior, cudaStream_t s) {
+  k_prior_bpd<<<B, 128, 0, s>>>(x0, sqrt_ac, log_1mac, t_last, per_scene, prior);
+}
+
+// ------------------------------------------------------------------------------------------------
 // p_losses value: one CTA (128 threads) per scene
 // parts[b] = {bbox, trans, size, angle, class, object, objfeat, liou, bbox_iou}
 // ------------------------------------------------------------------------------------------------
@@ -1432,7 +1527,10 @@ void init_pointwise_attrs() {
                                    cudaStream_t);                                                                 \
   template void launch_p_losses<T>(const float*, const float*, const float*, const T*, int, const int64_t*,       \
                                    const float*, const float*, const float*, const float*, const float*,          \
-                                   const float*, LossArgs, float*, float*, int, cudaStream_t);
+                                   const float*, LossArgs, float*, float*, int, cudaStream_t);                    \
+  template void launch_vlb_terms<T>(const StepCoef*, StepState*, const float*, const T*, int, const float*,      \
+                                    const float*, const float*, float*, float*, int, int, int, int, int,          \
+                                    cudaStream_t);
 INST(float)
 INST(bf16)
 

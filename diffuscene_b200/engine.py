@@ -103,6 +103,9 @@ class DenoiserEngine:
             keep.append(a)
             setattr(s, f, C.cast(C.c_void_p(a.data_ptr()), C.POINTER(C.c_float)))
         capi.check(self.lib.ds_set_schedule(self.h, C.byref(s)))
+        vt = [tables[f].detach().to(dtype=torch.float32, device="cpu").contiguous()
+              for f in ("posterior_log_variance_clipped", "model_log_variance", "log_one_minus_alphas_cumprod")]
+        capi.check(self.lib.ds_set_vlb_schedule(self.h, tables.T, *[_ptr(a) for a in vt]))
         self.tables = tables
 
     def set_context(self, context: torch.Tensor, shared: Optional[bool] = None):
@@ -226,6 +229,30 @@ class DenoiserEngine:
         capi.check(self.lib.ds_p_losses(self.h, _ptr(x0), _ptr(t), _ptr(noise), int(loss_separate), int(loss_iou),
                                         barr, _ptr(losses), _ptr(ld), B, self._stream()))
         return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}
+
+    # ---- variational bound ----------------------------------------------------------------------
+    def vlb(self, x0: torch.Tensor, clip_denoised: bool = True, seed: int = 0, scene_offset: int = 0,
+            noise: Optional[torch.Tensor] = None, use_graph: bool = True, prior_only: bool = False):
+        """calc_bpd_loop (diffusion_ddpm.py:690-717) per scene: (vb [B, T], mse [B, T], prior [B]), fp32 device
+        tensors, vb / prior in bits per dimension.  The q_sample draws come from Philox (seed, scene_offset + b) or from
+        `noise` [T, B, N, d] in loop order T-1 .. 0.  prior_only: just _prior_bpd (:679-688), no denoiser pass; vb and
+        mse are then None.  Conditioning is what set_context / set_context_cross last set."""
+        dev = self.device
+        x0 = x0.detach().to(device=dev, dtype=torch.float32).contiguous()
+        B = x0.shape[0]
+        noise = None if noise is None else noise.detach().to(device=dev, dtype=torch.float32).contiguous()
+        a = capi.DsVlbArgs()
+        a.batch, a.clip_denoised, a.x0_dev = B, int(bool(clip_denoised)), x0.data_ptr()
+        a.seed, a.scene_offset = int(seed), int(scene_offset)
+        a.noise_dev = None if noise is None else noise.data_ptr()
+        a.use_graph = int(use_graph)
+        T = self.num_timesteps
+        vb = None if prior_only else torch.empty((B, T), device=dev, dtype=torch.float32)
+        mse = None if prior_only else torch.empty((B, T), device=dev, dtype=torch.float32)
+        prior = torch.empty(B, device=dev, dtype=torch.float32)
+        torch.cuda.current_stream(dev).synchronize()
+        capi.check(self.lib.ds_vlb_loop(self.h, C.byref(a), _ptr(vb), _ptr(mse), _ptr(prior), None))
+        return vb, mse, prior
 
     # ---- native training ------------------------------------------------------------------------
     def flat_layout(self, prefix: str = "diffusion.model.") -> Dict[str, tuple]:

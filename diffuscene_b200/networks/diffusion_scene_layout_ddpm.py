@@ -4,7 +4,8 @@
 Same constructor arguments, same public methods (`get_loss`, `sample`, `generate_layout`,
 `generate_layout_progressive`, `complete_scene`, `arrange_scene`, `delete_empty_from_network_samples`,
 `delete_empty_boxes`) and the same state-dict key names (`positional_embedding`, `diffusion.model.*`,
-`fc_*`), so reference checkpoints load unchanged.  Parameters are fp32 `nn.Parameter`s (the master copy the
+`fc_*`), so reference checkpoints load unchanged.  The `diffusion` child carries the reference DiffusionPoint's
+likelihood methods, `prior_kl` and `all_kl` (the variational bound, `ds_vlb_loop`).  Parameters are fp32 `nn.Parameter`s (the master copy the
 optimizer updates); the engine keeps a packed copy that is refreshed lazily when the parameters change.
 
 Sampling, validation loss and every diffusion step run in the CUDA library, and so does training: forward and
@@ -19,6 +20,7 @@ batch_size > 1 via `delete_empty_batched` (the reference looks at batch row 0 on
 """
 from __future__ import annotations
 
+import weakref
 from typing import Dict, List, Optional
 
 import torch
@@ -36,6 +38,52 @@ from .functional import DenoiserFn
 
 class _Tree(nn.Module):
     """Plain container whose children are created on demand from dotted parameter names."""
+
+
+class _Diffusion(_Tree):
+    """The model's `diffusion` child: holds the denoiser parameters (`diffusion.model.*`, the reference checkpoint
+    names) and the likelihood methods of the reference's DiffusionPoint, `prior_kl` and `all_kl`
+    (diffusion_ddpm.py:734-745), which run in the CUDA library (ds_vlb_loop).  It adds no parameter, buffer or
+    state-dict key: the owning model is reached through a weak reference, not as a submodule."""
+
+    def __init__(self, owner: nn.Module):
+        super().__init__()
+        self._owner = weakref.ref(owner)
+
+    def __getstate__(self):      # a copy must not point at the original: the owner re-binds itself in __setstate__
+        state = self.__dict__.copy()
+        state["_owner"] = None
+        return state
+
+    def _model(self) -> "DiffusionSceneLayout_DDPM":
+        m = self._owner() if self._owner is not None else None
+        if m is None:
+            raise RuntimeError("the model owning this diffusion container no longer exists")
+        return m
+
+    @torch.no_grad()
+    def prior_kl(self, x0: torch.Tensor) -> torch.Tensor:
+        """_prior_bpd (:679-688): KL(q(x_{T-1} | x0) || N(0, I)) per scene, bits per dimension, [B]."""
+        return self._model().engine().vlb(x0, prior_only=True)[2]
+
+    @torch.no_grad()
+    def all_kl(self, x0: torch.Tensor, condition: torch.Tensor, condition_cross: Optional[torch.Tensor],
+               clip_denoised: bool = True, *, seed: Optional[int] = None, noise: Optional[torch.Tensor] = None):
+        """calc_bpd_loop (:690-717): the variational bound of the given scenes x0 [B, N, d] as the reference's dict of
+        four scalar means.  condition: the denoiser's context [B, N, E] or one [N, E] block shared by every scene;
+        condition_cross: the projected text [B, L, text_dim] of the text-conditioned networks (else None).  The
+        q_sample draws come from Philox keyed by `seed` (random when neither seed nor noise is given) or from `noise`
+        [T, B, N, d] in loop order T-1 .. 0.  Per-(scene, t) values: DenoiserEngine.vlb."""
+        m = self._model()
+        eng = m.engine()
+        eng.set_context(condition, shared=condition.dim() == 2)
+        if m.text_condition:
+            eng.set_context_cross(condition_cross)
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if noise is None else 0
+        vb, mse, prior = eng.vlb(x0, clip_denoised=clip_denoised, seed=seed, noise=noise)
+        return {"total_bpd_b": (vb.sum(dim=1) + prior).mean(), "terms_bpd": vb.mean(), "prior_bpd_b": prior.mean(),
+                "mse_bt": mse.mean()}
 
 
 def _register(root: nn.Module, dotted: str, param: nn.Parameter):
@@ -150,6 +198,7 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         # ---- denoiser parameters under the reference's names ("diffusion.model.*") ----
         self.spec = NetSpec.from_net_kwargs(config["net_kwargs"])
         self._param_names: List[str] = []
+        self.diffusion = _Diffusion(self)
         seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item())      # follows torch.manual_seed like nn init does
         for name, shape, kind in unet1d_param_specs(self.spec):
             _register(self, name, nn.Parameter(seeded_tensor(name, shape, kind, seed, perturb_norms=False)))
@@ -185,6 +234,10 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         self._weights_version = 0
         self._engine_version = -1
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_weights_dirty())
+
+    def __setstate__(self, state):
+        super().__setstate__(state)
+        self.diffusion._owner = weakref.ref(self)      # copies and unpickled models own their own container
 
     # ---- checkpoints ----------------------------------------------------------------------------
     FROZEN_PREFIXES = ("bertmodel.", "clip_model.", "feature_extractor.", "fc_room_f.")

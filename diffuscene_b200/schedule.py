@@ -70,6 +70,9 @@ def make_tables(betas: np.ndarray, mean_type: str = "eps", var_type: str = "fixe
         "posterior_variance": post_var, "posterior_log_variance_clipped": post_logvar,
         "coef1": b * torch.sqrt(ac_prev) / (1.0 - ac), "coef2": (1.0 - ac_prev) * torch.sqrt(a) / (1.0 - ac),
         "sigma": sigma, "loss_weight": lw,
+        # variational bound (ds_set_vlb_schedule): q_mean_variance's log-variance (:179) and p_mean_variance's model
+        # log-variance (:314-323), whose t = 0 entry `sigma` does not keep
+        "log_one_minus_alphas_cumprod": torch.log(1.0 - ac), "model_log_variance": logvar,
     }
     return DiffusionTables(T=len(betas64), mean_type=mean_type, var_type=var_type,
                            tables={k: v.float().contiguous() for k, v in t.items()})

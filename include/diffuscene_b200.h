@@ -119,6 +119,12 @@ typedef struct ds_schedule {
   const float* loss_weight;          /* p_losses weight per t (:194-203) */
 } ds_schedule;
 DS_API int ds_set_schedule(ds_handle* h, const ds_schedule* s);
+/* The extra tables of the variational bound (ds_vlb_loop), T fp32 host entries each, of the same schedule:
+ * post_logvar = posterior_log_variance_clipped (:190), model_logvar = the model log-variance of model_var_type
+ * (:314-323; fixedsmall: the same table, fixedlarge: log(cat(posterior_variance[1:2], betas[1:]))) and
+ * log_1mac = log_one_minus_alphas_cumprod (:179).  Kept apart from ds_schedule, whose layout is ABI. */
+DS_API int ds_set_vlb_schedule(ds_handle* h, int32_t T, const float* post_logvar, const float* model_logvar,
+                               const float* log_1mac);
 
 /* ---- conditioning -------------------------------------------------------------------------
  * `context` is the [B, N, cond_dim] tensor handed to Unet1D.forward (denoise_net.py:507, built at
@@ -168,6 +174,29 @@ DS_API int ds_traj_count(int32_t T, int32_t freq);
 /* One reverse step with explicit per-sample t (p_sample, diffusion_ddpm.py:339-352). */
 DS_API int ds_p_sample_step(ds_handle* h, const float* x_t_dev, const int64_t* t_dev, const float* noise_dev,
                      int32_t clip_denoised, float* out_dev, int32_t batch, void* stream);
+
+/* ---- variational bound --------------------------------------------------------------------
+ * Replaces GaussianDiffusion.calc_bpd_loop and _prior_bpd (diffusion_ddpm.py:679-717, behind DiffusionPoint.all_kl /
+ * prior_kl :734-745): for t = T-1 .. 0, x_t = q_sample(x0, t) -> denoiser -> vb[b][t] = mean over N*d of
+ * normal_kl(true posterior, model posterior) / ln 2 (:511-518) and mse[b][t] = mean (x0_hat - x0)^2, with x0_hat
+ * clamped when clip_denoised; prior[b] = _prior_bpd.  Like ds_sample_loop: one CUDA graph per step replayed T times
+ * (its own cached graph: a VLB call does not evict the sampling graph), t and the Philox state on the device, each
+ * scene's numbers independent of the batch it runs in.  Conditioning comes from ds_set_context /
+ * ds_set_context_cross with the same batch rules as sampling.  vb_dev and mse_dev ([batch, T] fp32 device) may both be
+ * NULL: then only prior_dev ([batch]) is computed, with no denoiser pass.  At t = 0 the reference compares against a
+ * posterior variance clipped to 1e-20, so for fixedsmall vb[b][0] ~ 0.5e20 * mean (x0 - x0_hat)^2 / ln 2. */
+typedef struct ds_vlb_args {
+  int32_t batch;
+  int32_t clip_denoised;        /* clamp the x0 estimate to [-1, 1] (:310-311)                                   */
+  const float* x0_dev;          /* [B, N, d] clean scenes                                                        */
+  uint64_t seed;                /* Philox seed of the q_sample draws when no noise is injected                   */
+  uint64_t scene_offset;        /* global index of scene 0 (RNG streams independent of sharding)                  */
+  const float* noise_dev;       /* optional injected q_sample noise [T, B, N, d], loop order T-1 .. 0             */
+  int32_t use_graph;            /* 1: CUDA-graph the step (default); 0: plain launches                            */
+  int32_t reserved[7];
+} ds_vlb_args;
+DS_API int ds_vlb_loop(ds_handle* h, const ds_vlb_args* a, float* vb_dev, float* mse_dev, float* prior_dev,
+                       void* stream);
 
 /* ---- training-side forward pieces ---------------------------------------------------------
  * q_sample (diffusion_ddpm.py:276-286) and the p_losses value (:520-652, loss.py:7-102): per-sample
