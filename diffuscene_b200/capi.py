@@ -41,6 +41,11 @@ class DsSampleArgs(C.Structure):
         ("chunk_scenes", C.c_int32), ("reserved", C.c_int32 * 5)]
 
 
+class DsRoomEncConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("precision", "input_channels", "height", "width", "device")] + \
+        [("reserved", C.c_int32 * 3)]
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -105,6 +110,12 @@ def load(rebuild: bool = False):
         "ds_graph_build_count": (C.c_int64, [H]),
         "ds_profile_ops": (C.c_int, [H, C.c_int32, C.c_char_p, C.c_int64, p, C.c_int32]),
         "ds_test_gemm_bf16": (C.c_int, [C.c_int, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p]),
+        "ds_room_enc_create": (C.c_int, [C.POINTER(DsRoomEncConfig), C.POINTER(H)]),
+        "ds_room_enc_destroy": (C.c_int, [H]),
+        "ds_room_enc_expected_weight_count": (C.c_int, [H]),
+        "ds_room_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+        "ds_room_enc_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, p]),
+        "ds_room_enc_backward": (C.c_int, [H, p, p, p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -121,7 +132,8 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_sample_loop_host", "ds_traj_count", "ds_p_sample_step", "ds_q_sample", "ds_p_losses", "ds_retrieve_objects",
             "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_sumsq", "ds_adam_step",
             "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
-            "ds_test_gemm_bf16"]
+            "ds_test_gemm_bf16", "ds_room_enc_create", "ds_room_enc_destroy", "ds_room_enc_expected_weight_count",
+            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward"]
 
 
 class DsError(RuntimeError):

@@ -121,6 +121,31 @@ void launch_retrieve(const int* class_start, int n_classes, const float* cat_fea
                      int size_dim, const int64_t* q_label, const float* q_feat, const float* q_size, int Q, int mode,
                      int64_t* out, cudaStream_t s);
 
+// ---- floor-plan encoder (room_encoder.cu): NHWC activation rows (scene, y, x) x channels ---------------------
+// One convolution: input [B * hin * win, cin] -> output [B * hout * wout, cout]; im2col columns (ky, kx, cin),
+// zero-padded to Kp (a multiple of 64).
+struct RoomConvGeom { int cin, cout, k, stride, pad, hin, win, hout, wout, Kp; };
+template <typename T> void launch_re_pack_mask(const float* mask, T* out, int B, int C, int H, int W, cudaStream_t s);
+template <typename T> void launch_re_im2col(const T* in, const RoomConvGeom& g, int B, T* cols, cudaStream_t s);
+// gather adjoint of im2col: out (= | +=) col2im(dcols) (+ add), zeroed where mask <= 0 (add / mask optional)
+template <typename T>
+void launch_re_col2im(const T* dcols, const RoomConvGeom& g, int B, T* out, int accumulate, const T* add, const T* mask,
+                      cudaStream_t s);
+template <typename T> void launch_re_add_relu(const T* z, const T* res, T* out, int64_t n, cudaStream_t s);
+// 3x3 / stride 2 / pad 1 max pool (torch's first-maximum argmax) and its gather adjoint (zeroed where in <= 0)
+template <typename T> void launch_re_maxpool(const T* in, T* out, int B, int C, int hin, int win, int hout, int wout, cudaStream_t s);
+template <typename T>
+void launch_re_maxpool_bwd(const T* in, const T* dout, T* din, int B, int C, int hin, int win, int hout, int wout,
+                           cudaStream_t s);
+template <typename T> void launch_re_avgpool(const T* in, float* feat, int B, int C, int hw, cudaStream_t s);
+template <typename T> void launch_re_avgpool_bwd(const float* dfeat, const T* out, T* d, int B, int C, int hw, cudaStream_t s);
+// FrozenBatchNorm fold (bn = weight, bias, running_mean, running_var of cout floats each) and its adjoint:
+// dW [cout, cin, k, k], dbn = [d weight | d bias]
+template <typename T>
+void launch_re_fold(const float* W, const float* bn, const RoomConvGeom& g, T* wp, float* bias, cudaStream_t s);
+void launch_re_fold_bwd(const float* dwp, const float* dbias, const float* W, const float* bn, const RoomConvGeom& g,
+                        float* dW, float* dbn, cudaStream_t s);
+
 // ---- GEMMs: D[M,N] = act([A0 | A1][M, K0+K1] * W[N, K0+K1]^T + bias) (+ residual) -----------------
 struct GemmArgs {
   const void* a0; int lda0; int k0;

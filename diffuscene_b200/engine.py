@@ -119,6 +119,9 @@ class DenoiserEngine:
             if shared:
                 context = context[0]
         ctx = context.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        # with torch on its default stream the library works on its own non-blocking stream, which does not wait for
+        # the kernels that produced `context`: let them finish first
+        torch.cuda.current_stream(self.device).synchronize()
         capi.check(self.lib.ds_set_context(self.h, _ptr(ctx), batch, int(bool(shared)), self._stream()))
         torch.cuda.current_stream(self.device).synchronize()
 
@@ -127,6 +130,7 @@ class DenoiserEngine:
             capi.check(self.lib.ds_set_context_cross(self.h, None, 0, 0, self._stream()))
             return
         c = cross.detach().to(device=self.device, dtype=torch.float32).contiguous()
+        torch.cuda.current_stream(self.device).synchronize()      # as in set_context
         capi.check(self.lib.ds_set_context_cross(self.h, _ptr(c), c.shape[0], c.shape[1], self._stream()))
         torch.cuda.current_stream(self.device).synchronize()
 

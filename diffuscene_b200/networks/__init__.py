@@ -29,12 +29,12 @@ def optimizer_factory(config, parameters):
 
 def build_network(input_dims, n_classes, config, weight_file=None, device="cpu", precision="bf16",
                   gemm_backend="auto"):
-    """Reference :37-68.  `feature_extractor` configs are accepted and ignored (only used when
-    room_mask_condition is true, which no shipped config sets)."""
+    """Reference :37-68.  The `feature_extractor` section configures the floor-plan encoder of networks with
+    room_mask_condition (ignored otherwise)."""
     network_type = config["network"]["type"]
     if network_type == "diffusion_scene_layout_ddpm":
-        network = DiffusionSceneLayout_DDPM(n_classes, None, config["network"], precision=precision,
-                                            gemm_backend=gemm_backend)
+        network = DiffusionSceneLayout_DDPM(n_classes, config.get("feature_extractor"), config["network"],
+                                            precision=precision, gemm_backend=gemm_backend)
     else:
         raise NotImplementedError()
     if weight_file is not None:

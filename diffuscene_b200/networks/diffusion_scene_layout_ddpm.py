@@ -30,10 +30,11 @@ from torch.nn.utils import clip_grad_norm_
 from ..engine import DenoiserEngine
 from ..optim import NativeAdam
 from ..parallel import allreduce_flat, allreduce_gradients
+from ..room_encoder import RoomEncoderFn, RoomMaskEncoder, trunk_specs
 from ..schedule import get_betas, make_tables
 from ..stats_logger import StatsLogger
 from ..weights import NetSpec, seeded_tensor, unet1d_param_specs
-from .functional import DenoiserFn
+from .functional import DenoiserFn, room_trunk
 
 
 class _Tree(nn.Module):
@@ -86,14 +87,54 @@ class _Diffusion(_Tree):
                 "mse_bt": mse.mean()}
 
 
-def _register(root: nn.Module, dotted: str, param: nn.Parameter):
+def _register(root: nn.Module, dotted: str, param: nn.Parameter, buffer: bool = False):
     parts = dotted.split(".")
     mod = root
     for part in parts[:-1]:
         if part not in mod._modules:
             mod.add_module(part, _Tree())
         mod = mod._modules[part]
-    mod.register_parameter(parts[-1], param)
+    if buffer:
+        mod.register_buffer(parts[-1], param)
+    else:
+        mod.register_parameter(parts[-1], param)
+
+
+ROOM_TRUNK = "feature_extractor._feature_extractor."
+
+
+def _room_feature_extractor(fe_config, freeze_bn_default=True) -> nn.Module:
+    """The reference's ResNet18 feature extractor (feature_extractors.py:19-47) as a module tree with its parameter
+    and buffer names: the trunk's tensors are plain parameters / buffers (the CUDA encoder computes with them), the
+    fc head is an ordinary torch Sequential.  Initialised like torchvision's resnet18 (kaiming-normal convs, unit
+    BatchNorm scale) with the eps folded into running_var as FrozenBatchNorm2d.from_batch_norm does."""
+    fe_config = dict(fe_config or {})
+    name = fe_config.get("name", "resnet18")
+    if name != "resnet18":
+        raise NotImplementedError("floor-plan feature extractor %r: only resnet18 has a native encoder" % name)
+    if not fe_config.get("freeze_bn", freeze_bn_default):
+        raise NotImplementedError("freeze_bn: false (train-mode BatchNorm couples the scenes of a batch); the native "
+                                  "floor-plan encoder supports the frozen BatchNorm every config uses")
+    cin = int(fe_config.get("input_channels", 1))
+    feature_size = int(fe_config.get("feature_size", 256))
+    root = _Tree()
+    fe = _Tree()
+    root.add_module("feature_extractor", fe)
+    for name, shape, is_buf in trunk_specs(cin):
+        if name.endswith("running_var"):
+            v = torch.full(shape, 1.0 + 1e-5)
+        elif name.endswith("running_mean") or name.endswith(".bias"):
+            v = torch.zeros(shape)
+        elif len(shape) == 1:
+            v = torch.ones(shape)
+        else:
+            v = torch.empty(shape)
+            nn.init.kaiming_normal_(v, mode="fan_out", nonlinearity="relu")
+        _register(root, ROOM_TRUNK + name, v if is_buf else nn.Parameter(v), buffer=is_buf)
+    fe._feature_extractor.add_module("fc", nn.Sequential(nn.Linear(512, 512), nn.ReLU(), nn.Linear(512, feature_size)))
+    fe.feature_size = feature_size
+    fe.input_channels = cin
+    return fe
 
 
 class _NativeTrainLoss(torch.autograd.Function):
@@ -125,9 +166,13 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         self.text_glove_embedding = config.get("text_glove_embedding", False)
         self.text_clip_embedding = config.get("text_clip_embedding", False)
         if self.room_mask_condition:
-            raise NotImplementedError("room_mask_condition (floor-plan encoder) is outside the hot path; every "
-                                      "shipped config sets it to false")
-        if self.text_condition:
+            if self.text_condition:
+                raise NotImplementedError("room_mask_condition together with text_condition: the reference builds no "
+                                          "text modules in that case (its `elif`, diffusion_scene_layout_ddpm.py:33)")
+            # `feature_extractor`: the `feature_extractor:` section of the config (build_network passes it through)
+            self.feature_extractor = _room_feature_extractor(feature_extractor)
+            self.fc_room_f = nn.Linear(self.feature_extractor.feature_size, config["latent_dim"])
+        elif self.text_condition:
             text_embed_dim = config.get("text_embed_dim", 512)
             if self.text_glove_embedding:
                 self.fc_text_f = nn.Linear(50, text_embed_dim)
@@ -233,6 +278,9 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         self.native_backward = True      # False: differentiate functional.DenoiserFn with torch autograd instead
         self._weights_version = 0
         self._engine_version = -1
+        self._room_enc: Optional[RoomMaskEncoder] = None
+        self._room_flat = None
+        self._room_grads = None
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.mark_weights_dirty())
 
     def __setstate__(self, state):
@@ -247,7 +295,9 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         registers it as a submodule, diffusion_scene_layout_ddpm.py:47-48); those keys are dropped here -- the
         encoder is loaded from its own pretrained files -- so that `strict=True` keeps checking everything that
         is trained on this path."""
-        sd = {k: v for k, v in state_dict.items() if not k.startswith(self.FROZEN_PREFIXES)}
+        drop = tuple(p for p in self.FROZEN_PREFIXES
+                     if not (self.room_mask_condition and p in ("feature_extractor.", "fc_room_f.")))
+        sd = {k: v for k, v in state_dict.items() if not k.startswith(drop)}
         return super().load_state_dict(sd, strict=strict, **kw)
 
     # ---- engine management ----------------------------------------------------------------------
@@ -342,6 +392,76 @@ class DiffusionSceneLayout_DDPM(nn.Module):
                 p.grad = p.grad + view
         self._native_grads_ready = True
 
+    # ---- floor-plan encoder ---------------------------------------------------------------------------
+    def _room_tensors(self) -> Dict[str, torch.Tensor]:
+        """Trunk parameters and buffers by their names relative to ROOM_TRUNK, in the encoder's flat order."""
+        named = dict(self.named_parameters())
+        named.update(dict(self.named_buffers()))
+        return {n: named[ROOM_TRUNK + n] for n, _, _ in trunk_specs(self.feature_extractor.input_channels)}
+
+    def _ensure_room_flat(self, H: int, W: int) -> RoomMaskEncoder:
+        """The trunk's parameters and buffers as views into ONE flat fp32 device buffer (ds_room_enc_expected_weight
+        order), which the CUDA encoder reads; gradients go to a second flat buffer."""
+        dev = self._device()
+        cin = self.feature_extractor.input_channels
+        enc = self._room_enc
+        if enc is None or enc.device != dev or (enc.cfg.height, enc.cfg.width) != (H, W):
+            if enc is not None:
+                enc.close()
+            enc = self._room_enc = RoomMaskEncoder(cin, H, W, precision=self._precision, device=dev.index or 0)
+        tensors = self._room_tensors()
+        if self._room_flat is not None and self._room_flat.device == dev:
+            base, off, ok = self._room_flat.data_ptr(), 0, True
+            for t in tensors.values():
+                ok = ok and t.data_ptr() == base + 4 * off
+                off += t.numel()
+            if ok:
+                return enc
+        total = sum(t.numel() for t in tensors.values())
+        flat = torch.empty(total, device=dev, dtype=torch.float32)
+        off = 0
+        for name, t in tensors.items():
+            n = t.numel()
+            flat[off:off + n].copy_(t.detach().reshape(-1))
+            view = flat[off:off + n].view(t.shape)
+            if isinstance(t, nn.Parameter):
+                t.data = view
+            else:
+                mod = self.get_submodule((ROOM_TRUNK + name).rsplit(".", 1)[0])
+                mod._buffers[name.rsplit(".", 1)[1]] = view
+            off += n
+        self._room_flat = flat
+        self._room_grads = torch.zeros(total, device=dev, dtype=torch.float32)
+        return enc
+
+    def _room_features(self, room_mask: torch.Tensor) -> torch.Tensor:
+        """fc_room_f(feature_extractor(room_mask)) [B, latent_dim] (reference :162-164, :236-238).  The trunk runs in
+        the CUDA library; with native_backward = False and gradients enabled, functional.room_trunk under torch
+        autograd instead (the parity twin)."""
+        fe = self.feature_extractor._feature_extractor
+        room_mask = room_mask.to(self._device(), torch.float32)
+        if room_mask.dim() != 4:
+            raise ValueError("room mask must be [B, C, H, W], got %s" % (tuple(room_mask.shape),))
+        grad = torch.is_grad_enabled()
+        if grad and not self.native_backward:
+            feat = room_trunk(self._room_tensors(), room_mask)
+        else:
+            enc = self._ensure_room_flat(room_mask.shape[2], room_mask.shape[3])
+            if grad:
+                slices, params, off, tensors = [], [], 0, self._room_tensors()
+                for name, shape, is_buf in trunk_specs(self.feature_extractor.input_channels):
+                    n = 1
+                    for s in shape:
+                        n *= s
+                    if not is_buf:
+                        slices.append((off, n, shape))
+                        params.append(tensors[name])
+                    off += n
+                feat = RoomEncoderFn.apply(room_mask, enc, self._room_flat, self._room_grads, slices, *params)
+            else:
+                feat = enc.forward(self._room_flat, room_mask)
+        return self.fc_room_f(fe.fc(feat))
+
     def _denoiser_params(self) -> Dict[str, torch.Tensor]:
         pre = "diffusion.model."
         return {n[len(pre):]: p for n, p in self.named_parameters() if n.startswith(pre)}
@@ -355,11 +475,18 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         eye = torch.eye(self.sample_num_points, device=device)
         return self.fc_instance_condition(eye), True
 
-    def _condition(self, batch, device, layout_target=None, partial_boxes=None, input_boxes=None, num_points=None):
-        """Returns (condition [B,N,E] or [N,E], shared flag)."""
+    def _condition(self, batch, device, layout_target=None, partial_boxes=None, input_boxes=None, num_points=None,
+                   room_f=None):
+        """Returns (condition [B,N,E] or [N,E], shared flag).  room_f: the floor-plan feature [B, latent_dim], which
+        comes first in the condition (reference :184-191)."""
         inst, shared = self._instance_condition(batch, device)
         cond = inst
         N = num_points or self.sample_num_points
+        if room_f is not None:
+            r = room_f[:, None].expand(-1, N, -1)
+            if cond is not None:
+                r = torch.cat([r, cond[None].expand(batch, -1, -1) if cond.dim() == 2 else cond], dim=-1)
+            cond, shared = r, False
         if self.room_partial_condition:
             if partial_boxes is not None:
                 zeros = torch.zeros((batch, N - partial_boxes.shape[1], partial_boxes.shape[2]), device=device)
@@ -423,7 +550,8 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         target = self._pack_target(sample_params).float()
         B, N, _ = target.shape
         device = target.device
-        cond, shared = self._condition(B, device, layout_target=target)
+        room_f = self._room_features(sample_params["room_layout"]) if self.room_mask_condition else None
+        cond, shared = self._condition(B, device, layout_target=target, room_f=room_f)
         if self.room_arrange_condition:
             target = torch.cat([target[:, :, :self.translation_dim],
                                 target[:, :, self.translation_dim + self.size_dim:self.bbox_dim]], dim=-1).contiguous()
@@ -527,8 +655,14 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         device = room_mask.device if torch.is_tensor(room_mask) else self._device()
         if num_points != self.sample_num_points:
             raise ValueError("num_points must equal sample_num_points (%d)" % self.sample_num_points)
+        room_f = None
+        if self.room_mask_condition:
+            if not torch.is_tensor(room_mask) or room_mask.size(0) != batch_size:
+                raise ValueError("room_mask must hold one floor plan per scene: %s masks for batch_size %d" % (
+                    tuple(room_mask.shape)[:1] if torch.is_tensor(room_mask) else None, batch_size))
+            room_f = self._room_features(room_mask)
         cond, shared = self._condition(batch_size, device, partial_boxes=partial_boxes, input_boxes=input_boxes,
-                                       num_points=num_points)
+                                       num_points=num_points, room_f=room_f)
         eng = self.engine()
         eng.set_context(cond, shared=shared)
         if self.text_condition:

@@ -164,3 +164,29 @@ class DenoiserFn:
                 outs.append(self.mlp3("objfeat_hidden2output", h))
             return torch.cat(outs, dim=-1)
         return F.linear(h, _w(p["final_conv.weight"]), p["final_conv.bias"])
+
+
+def _frozen_bn(x, t, name):
+    """FrozenBatchNorm2d (reference frozen_batchnorm.py): no eps, it was folded into running_var when frozen."""
+    scale = t[name + ".weight"] * t[name + ".running_var"].rsqrt()
+    bias = t[name + ".bias"] - t[name + ".running_mean"] * scale
+    return x * scale.reshape(1, -1, 1, 1) + bias.reshape(1, -1, 1, 1)
+
+
+def room_trunk(t, x):
+    """The ResNet-18 trunk of the floor-plan encoder (torchvision resnet18 with the reference's conv1 and frozen
+    BatchNorm, feature_extractors.py:19-47) up to the global average pool: mask [B, C, H, W] -> [B, 512].  `t` maps the
+    names relative to `feature_extractor._feature_extractor.` to tensors.  The autograd twin of the CUDA encoder."""
+    x = F.relu(_frozen_bn(F.conv2d(x, t["conv1.weight"], stride=2, padding=3), t, "bn1"))
+    x = F.max_pool2d(x, 3, 2, 1)
+    for L in range(1, 5):
+        for j in range(2):
+            pre = "layer%d.%d." % (L, j)
+            stride = 2 if (L > 1 and j == 0) else 1
+            out = F.relu(_frozen_bn(F.conv2d(x, t[pre + "conv1.weight"], stride=stride, padding=1), t, pre + "bn1"))
+            out = _frozen_bn(F.conv2d(out, t[pre + "conv2.weight"], padding=1), t, pre + "bn2")
+            idn = x
+            if pre + "downsample.0.weight" in t:
+                idn = _frozen_bn(F.conv2d(x, t[pre + "downsample.0.weight"], stride=stride), t, pre + "downsample.1")
+            x = F.relu(out + idn)
+    return F.adaptive_avg_pool2d(x, 1).flatten(1)

@@ -3,7 +3,8 @@
 Produces the `sample_params` contract of `Diffusion.__getitem__` after `Scale_CosinAngle_ObjfeatsNorm`
 (reference scene_synthesis/datasets/threed_front_dataset.py:481-513, 888-925; SURVEY.md A.4) and its inverse
 `post_process` (:515-535): +-1 class one-hots whose last channel is the 'empty' slot, translations / sizes /
-objfeats in [-1, 1], angles as (cos, sin), a zero room layout.
+objfeats in [-1, 1], angles as (cos, sin), and a room layout: a seeded binary floor plan (rectangle or L-shape) for
+networks with room_mask_condition, zeros otherwise.
 """
 from __future__ import annotations
 
@@ -30,6 +31,22 @@ def write_stats_file(path, bounds=DEFAULT_BOUNDS):
     return path
 
 
+def floor_plan_mask(g: torch.Generator, size: int = 64) -> torch.Tensor:
+    """A binary floor plan [1, size, size]: an axis-aligned rectangular room, half of the time with one corner cut
+    away (an L-shape)."""
+    r = lambda lo, hi: int(torch.randint(lo, hi, (1,), generator=g))
+    y0, x0 = r(1, size // 3), r(1, size // 3)
+    y1, x1 = r(2 * size // 3, size), r(2 * size // 3, size)
+    m = torch.zeros(1, size, size)
+    m[:, y0:y1, x0:x1] = 1.0
+    if r(0, 2):
+        cy, cx = r(y0 + 2, y1 - 1), r(x0 + 2, x1 - 1)
+        ys = slice(y0, cy) if r(0, 2) else slice(cy, y1)
+        xs = slice(x0, cx) if r(0, 2) else slice(cx, x1)
+        m[:, ys, xs] = 0.0
+    return m
+
+
 class SyntheticScenes(Dataset):
     def __init__(self, net_cfg: dict, length: int = 4096, seed: int = 0, bounds=DEFAULT_BOUNDS):
         self.N = net_cfg.get("sample_num_points", 12)
@@ -37,6 +54,7 @@ class SyntheticScenes(Dataset):
         self.angle_dim = net_cfg.get("angle_dim", 1)
         self.objfeat_dim = net_cfg.get("objfeat_dim", 0)
         self.objectness_dim = net_cfg.get("objectness_dim", 1)
+        self.room_mask = net_cfg.get("room_mask_condition", True)
         self.length, self.seed, self.bounds = length, seed, bounds
         self.n_classes = self.class_dim + 1      # + start token, as the reference counts them
         self.feature_size = 8 + self.class_dim
@@ -61,6 +79,8 @@ class SyntheticScenes(Dataset):
             ang = th.expand(N, self.angle_dim) / 3.14159 * real
         out = {"class_labels": onehot, "translations": tr, "sizes": sz, "angles": ang,
                "room_layout": torch.zeros(1, 64, 64), "length": n_real}
+        if self.room_mask:      # a generator of its own: the other fields do not depend on whether masks are drawn
+            out["room_layout"] = floor_plan_mask(torch.Generator().manual_seed(self.seed * 1000003 + idx + (1 << 40)))
         if self.objfeat_dim > 0:
             key = "objfeats_32" if self.objfeat_dim == 32 else "objfeats"
             out[key] = (torch.rand(N, self.objfeat_dim, generator=g) * 2 - 1) * real

@@ -275,6 +275,39 @@ DS_API int ds_retrieve_objects(const int32_t* class_start_dev, int32_t n_classes
                                const int64_t* q_label_dev, const float* q_feat_dev, const float* q_size_dev,
                                int32_t num_queries, int32_t mode, int64_t* out_index_dev, void* stream);
 
+/* ---- floor-plan encoder --------------------------------------------------------------------
+ * Replaces the ResNet-18 trunk of the reference's room-mask feature extractor (scene_synthesis/networks/
+ * feature_extractors.py:19-47 with FrozenBatchNorm2d, frozen_batchnorm.py): conv1 -> bn1 -> ReLU -> maxpool ->
+ * layer1 .. layer4 -> global average pool, giving the [B, 512] input of its fc head.  The fc head and fc_room_f stay
+ * on the caller's side.  A handle of its own, independent of ds_handle.
+ * Parameters are ONE flat fp32 device buffer in ds_room_enc_expected_weight() order: the reference names under
+ * `feature_extractor._feature_extractor.` (conv1.weight, bn1.weight, bn1.bias, bn1.running_mean, bn1.running_var,
+ * layer1.0.conv1.weight, ...), the BatchNorm running statistics included.  The running variance already holds the
+ * eps (FrozenBatchNorm2d.from_batch_norm folds it in).  Buffers grow on the first call at a larger batch; after that
+ * nothing is allocated inside a call.  `stream` is used as given: NULL is the default stream, not a stream of the
+ * handle's own. */
+typedef struct ds_room_enc ds_room_enc;
+typedef struct ds_room_enc_config {
+  int32_t precision;        /* ds_precision: fp32 parity mode or bf16 tensor-core mode                      */
+  int32_t input_channels;   /* channels of the mask, 1 .. 8                                                  */
+  int32_t height, width;    /* mask size, each a multiple of 32 and at least 32 (64 x 64 in the reference)   */
+  int32_t device;           /* CUDA device ordinal                                                           */
+  int32_t reserved[3];
+} ds_room_enc_config;
+/* DS_ERR_INVALID for input_channels outside [1, 8] or a height / width below 32 or not a multiple of 32. */
+DS_API int ds_room_enc_create(const ds_room_enc_config* cfg, ds_room_enc** out);
+DS_API int ds_room_enc_destroy(ds_room_enc* h);
+DS_API int ds_room_enc_expected_weight_count(ds_room_enc* h);
+DS_API int ds_room_enc_expected_weight(ds_room_enc* h, int index, const char** name, int64_t* numel);
+/* mask [batch, input_channels, height, width] fp32 -> feat [batch, 512] fp32, device pointers.  A scene's features do
+ * not depend on the batch it runs in.  keep_for_backward != 0 keeps the activations, and the flat_params_dev pointer
+ * (which must stay valid and unchanged), for ds_room_enc_backward. */
+DS_API int ds_room_enc_forward(ds_room_enc* h, const float* flat_params_dev, const float* mask_dev, int32_t batch,
+                               float* feat_dev, int32_t keep_for_backward, void* stream);
+/* d(loss)/d(feat) [batch, 512] of the kept forward -> flat_grads_dev (same layout as the parameters, overwritten;
+ * the running statistics get 0).  DS_ERR_INVALID when no forward was kept. */
+DS_API int ds_room_enc_backward(ds_room_enc* h, const float* dfeat_dev, float* flat_grads_dev, void* stream);
+
 /* ---- introspection / debugging ------------------------------------------------------------ */
 /* Human-readable op list of the step program (works without a device when h == NULL: builds the plan
  * for `cfg` on the host only).  Returns bytes written (excluding NUL) or a negative status. */

@@ -48,7 +48,11 @@ def main(argv):
     done = 0
     while done < args.n_sequences:
         bs = min(args.batch_size, args.n_sequences - done)
-        room_mask = torch.zeros(bs, 1, 64, 64, device=device)
+        if network.room_mask_condition:      # floor-plan configs: the synthetic floor plans of these scenes
+            sds = SyntheticScenes(config["network"], args.n_sequences, seed=args.seed)
+            room_mask = torch.stack([sds[done + i]["room_layout"] for i in range(bs)]).to(device)
+        else:
+            room_mask = torch.zeros(bs, 1, 64, 64, device=device)
         samples = network.sample(room_mask, N, d, batch_size=bs, clip_denoised=args.clip_denoised, ddim=args.ddim,
                                  ddim_steps=args.ddim_steps, seed=args.seed * 100003 + done)
         for i, scene in enumerate(network.delete_empty_batched(samples)):
