@@ -46,6 +46,10 @@ class DsRoomEncConfig(C.Structure):
         [("reserved", C.c_int32 * 3)]
 
 
+class DsShapeAeConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("latent_dim", "num_points", "device")] + [("reserved", C.c_int32 * 5)]
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -116,6 +120,17 @@ def load(rebuild: bool = False):
         "ds_room_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
         "ds_room_enc_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, p]),
         "ds_room_enc_backward": (C.c_int, [H, p, p, p]),
+        "ds_shape_ae_create": (C.c_int, [C.POINTER(DsShapeAeConfig), C.POINTER(H)]),
+        "ds_shape_ae_destroy": (C.c_int, [H]),
+        "ds_shape_ae_expected_weight_count": (C.c_int, [H]),
+        "ds_shape_ae_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+        "ds_shape_ae_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p]),
+        "ds_shape_ae_train_step": (C.c_int, [H, p, p, C.c_int32, p, C.c_float, p, p, p]),
+        "ds_shape_ae_set_knn": (C.c_int, [H, p]),
+        "ds_shape_ae_get_knn": (C.c_int, [H, p, p]),
+        "ds_knn": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, p]),
+        "ds_chamfer_forward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p]),
+        "ds_chamfer_backward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p, p, p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -133,7 +148,10 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_sumsq", "ds_adam_step",
             "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
             "ds_test_gemm_bf16", "ds_room_enc_create", "ds_room_enc_destroy", "ds_room_enc_expected_weight_count",
-            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward"]
+            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_shape_ae_create",
+            "ds_shape_ae_destroy", "ds_shape_ae_expected_weight_count", "ds_shape_ae_expected_weight",
+            "ds_shape_ae_forward", "ds_shape_ae_train_step", "ds_shape_ae_set_knn", "ds_shape_ae_get_knn", "ds_knn",
+            "ds_chamfer_forward", "ds_chamfer_backward"]
 
 
 class DsError(RuntimeError):

@@ -190,3 +190,93 @@ def room_trunk(t, x):
                 idn = _frozen_bn(F.conv2d(x, t[pre + "downsample.0.weight"], stride=stride), t, pre + "downsample.1")
             x = F.relu(out + idn)
     return F.adaptive_avg_pool2d(x, 1).flatten(1)
+
+
+# ---- object shape auto-encoder (reference foldingnet_autoencoder.py:131-390) --------------------------------------------
+def shape_ae_grid(device=None) -> torch.Tensor:
+    """The decoder's fixed 2 x 2025 grid: np.meshgrid(linspace(-0.3, 0.3, 45) x 2), flattened (:253-258)."""
+    import numpy as np
+    xx = np.linspace(-0.3, 0.3, 45, dtype=np.float32)
+    return torch.from_numpy(np.stack(np.meshgrid(xx, xx)).reshape(2, -1)).to(device)
+
+
+def knn_reference(x, k: int = 16):
+    """The reference's kNN (:59-76): x [B, C, N] -> [B, N, k], topk of the negated squared distance in its expanded
+    form.  The order of equal distances is torch's; the CUDA kernel breaks ties by the lower index."""
+    inner = -2 * torch.matmul(x.transpose(2, 1), x)
+    xx = torch.sum(x ** 2, dim=1, keepdim=True)
+    return (-xx - inner - xx.transpose(2, 1)).topk(k=k, dim=-1)[1]
+
+
+def _gather_points(x, idx):
+    """x [B, C, N], idx [B, N, k] -> [B, N, k, C] (index_points of :39-56)."""
+    B, N, k = idx.shape
+    pts = x.permute(0, 2, 1)
+    return torch.gather(pts, 1, idx.reshape(B, -1, 1).expand(-1, -1, pts.shape[-1])).reshape(B, N, k, -1)
+
+
+def _bn1d(x, t, name, train):
+    return F.batch_norm(x, t[name + ".running_mean"], t[name + ".running_var"], t[name + ".weight"], t[name + ".bias"],
+                        training=train, momentum=0.1, eps=1e-5)
+
+
+def _conv1d(x, t, name):
+    return F.conv1d(x, t[name + ".weight"], t[name + ".bias"])
+
+
+def shape_ae_forward(t, points, eps, knn=None, train: bool = True):
+    """The autograd twin of the CUDA shape auto-encoder: points [B, P, 3], eps [B, F] -> dict of kl [B], latent [B, F],
+    recon [B, 2025, 3], the three stages' kNN indices (`knn`) and the features they searched (`knn_inputs`, [B, P, C]).  `t` maps the reference's state-dict names to tensors; in
+    train mode BatchNorm uses batch statistics and updates the running statistics in `t` in place.  `knn` (three
+    [B, P, 16] index tensors) replaces the kNN searches."""
+    x = points.permute(0, 2, 1)
+    b, _, n = x.shape
+    used, inputs = [], []
+
+    def nbrs(feat, stage):
+        idx = knn_reference(feat) if knn is None else knn[stage].to(feat.device, torch.long)
+        used.append(idx)
+        inputs.append(feat.detach().permute(0, 2, 1))
+        return _gather_points(feat, idx)
+
+    knn_x = nbrs(x, 0)
+    knn_x = knn_x - knn_x.mean(dim=2, keepdim=True)
+    cov = torch.matmul(knn_x.permute(0, 1, 3, 2), knn_x).view(b, n, -1).permute(0, 2, 1)
+    h = torch.cat([x, cov], dim=1)
+    for i in (1, 2, 3):
+        h = F.relu(_bn1d(_conv1d(h, t, "encoder.conv%d" % i), t, "encoder.bn%d" % i, train))
+    for g in (1, 2):
+        h = torch.max(nbrs(h, g), dim=2)[0].permute(0, 2, 1)
+        pre = "encoder.graph_layer%d" % g
+        h = F.relu(_bn1d(_conv1d(h, t, pre + ".conv"), t, pre + ".bn", train))
+    code = torch.max(_bn1d(_conv1d(h, t, "encoder.conv4"), t, "encoder.bn4", train), dim=-1)[0]
+    mean = F.linear(code, t["mean_fc.weight"], t["mean_fc.bias"])
+    logvar = torch.clamp(F.linear(code, t["logvar_fc.weight"], t["logvar_fc.bias"]), -30.0, 20.0)
+    lat = mean + torch.exp(0.5 * logvar) * eps
+    kl = 0.5 * torch.mean(torch.pow(mean, 2) + torch.exp(logvar) - 1.0 - logvar, dim=[1])
+    code = F.linear(lat, t["fc.weight"], t["fc.bias"])[:, :, None].repeat(1, 1, 2025)
+    rec = shape_ae_grid(points.device)[None].repeat(b, 1, 1)
+    for f in ("fold1", "fold2"):
+        pre = "decoder.%s.layers." % f
+        z = torch.cat([rec, code], dim=1)
+        z = F.relu(_bn1d(_conv1d(z, t, pre + "0"), t, pre + "1", train))
+        z = F.relu(_bn1d(_conv1d(z, t, pre + "3"), t, pre + "4", train))
+        rec = _conv1d(z, t, pre + "6")
+    return {"kl": kl, "latent": lat, "recon": rec.permute(0, 2, 1), "knn": used, "knn_inputs": inputs}
+
+
+def chamfer_torch(a, b):
+    """chamfer_3DDist restated with torch ops: a [B, n, 3], b [B, m, 3] -> dist1 [B, n], dist2 [B, m], idx1, idx2
+    (int32), squared distances in the difference form."""
+    d = ((a[:, :, None, :] - b[:, None, :, :]) ** 2).sum(-1)
+    d1, i1 = d.min(dim=2)
+    d2, i2 = d.min(dim=1)
+    return d1, d2, i1.int(), i2.int()
+
+
+def shape_ae_loss(out, points, kl_weight):
+    """get_loss (:374-390) on the twin's outputs: (loss, loss_cd, loss_kl)."""
+    d1, d2, _, _ = chamfer_torch(points, out["recon"])
+    loss_kl = torch.sum(out["kl"]) / out["kl"].shape[0]
+    loss_cd = (d1.mean(dim=1) + d2.mean(dim=1)).mean()
+    return loss_cd + loss_kl * kl_weight, loss_cd, loss_kl

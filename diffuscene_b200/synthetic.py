@@ -107,3 +107,33 @@ class SyntheticScenes(Dataset):
             else:
                 out[k] = self.descale(v, self.bounds[k][0], self.bounds[k][1])
         return out
+
+
+class SyntheticShapes(Dataset):
+    """Stand-in for the reference's object point-cloud dataset (threed_future_dataset.py:100-120, 3D-FUTURE is licensed
+    and absent here): seeded boxes and ellipsoids with random proportions, surface-sampled densely, centred and scaled
+    into the unit sphere, from which `num_points` points are drawn WITH replacement as the reference does, so a cloud
+    holds exact duplicate points.  Items are {"points": [P, 3] fp32, "label": int, "size": [3] fp32}."""
+
+    N_DENSE = 4096
+
+    def __init__(self, length: int = 1024, num_points: int = 2048, seed: int = 0, n_classes: int = 2):
+        self.length, self.num_points, self.seed, self.n_classes = length, num_points, seed, n_classes
+
+    def __len__(self):
+        return self.length
+
+    def __getitem__(self, i):
+        g = torch.Generator().manual_seed(self.seed * 1000003 + i)
+        label = int(torch.randint(0, self.n_classes, (1,), generator=g))
+        half = 0.2 + torch.rand(3, generator=g)
+        u = torch.randn(self.N_DENSE, 3, generator=g)
+        if label % 2 == 0:      # box: project onto the face of the largest normalised coordinate
+            u = u / u.abs().amax(dim=1, keepdim=True)
+        else:                   # ellipsoid
+            u = u / u.norm(dim=1, keepdim=True)
+        dense = u * half
+        dense = dense - dense.mean(dim=0)
+        dense = dense / dense.norm(dim=1).max()
+        pick = torch.randint(0, self.N_DENSE, (self.num_points,), generator=g)
+        return {"points": dense[pick].float().contiguous(), "label": label, "size": (2 * half).float()}

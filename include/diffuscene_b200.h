@@ -308,7 +308,63 @@ DS_API int ds_room_enc_forward(ds_room_enc* h, const float* flat_params_dev, con
  * the running statistics get 0).  DS_ERR_INVALID when no forward was kept. */
 DS_API int ds_room_enc_backward(ds_room_enc* h, const float* dfeat_dev, float* flat_grads_dev, void* stream);
 
+/* ---- object shape auto-encoder ---------------------------------------------------------------
+ * The reference's KLAutoEncoder (scene_synthesis/networks/foldingnet_autoencoder.py:131-390): a FoldingNet encoder
+ * (kNN covariances, three 1x1 convs, two kNN graph layers, conv4, max over the points), a KL latent head and a
+ * two-stage folding decoder onto a fixed 45 x 45 grid, trained with the Chamfer distance.  fp32 throughout.  A handle
+ * of its own, independent of ds_handle.
+ * Parameters are ONE flat fp32 device buffer in ds_shape_ae_expected_weight() order: the reference's state-dict names
+ * (encoder.conv1.weight, ..., decoder.fold2.layers.6.bias) with the BatchNorm running statistics included and
+ * num_batches_tracked left out.  Points are [batch, num_points, 3], the latent and eps [batch, latent_dim], kl
+ * [batch], the reconstruction [batch, 2025, 3]; all device pointers.  Buffers grow on the first call at a larger
+ * batch; `stream` is used as given. */
+typedef struct ds_shape_ae ds_shape_ae;
+typedef struct ds_shape_ae_config {
+  int32_t latent_dim;       /* objfeat_dim of the reference config, 1 .. 512 (32 or 64 in the shipped configs)      */
+  int32_t num_points;       /* points per object, at least 16 (2048 in the reference's dataset)                   */
+  int32_t device;           /* CUDA device ordinal                                                                */
+  int32_t reserved[5];
+} ds_shape_ae_config;
+/* DS_ERR_INVALID for latent_dim outside [1, 512] or num_points < 16. */
+DS_API int ds_shape_ae_create(const ds_shape_ae_config* cfg, ds_shape_ae** out);
+DS_API int ds_shape_ae_destroy(ds_shape_ae* h);
+DS_API int ds_shape_ae_expected_weight_count(ds_shape_ae* h);
+DS_API int ds_shape_ae_expected_weight(ds_shape_ae* h, int index, const char** name, int64_t* numel);
+/* kl, latent = mean + exp(logvar / 2) eps and the reconstruction of `points` (each output optional).  eps is the
+ * caller's N(0, 1) draw.  train != 0: BatchNorm uses batch statistics and updates the running statistics inside
+ * flat_params_dev; train == 0: running statistics, and an object's outputs do not depend on the batch it runs in.
+ * keep != 0 keeps this pass readable through ds_shape_ae_get_knn. */
+DS_API int ds_shape_ae_forward(ds_shape_ae* h, float* flat_params_dev, const float* points_dev, int32_t batch,
+                               const float* eps_dev, int32_t train, int32_t keep, float* latent_dev, float* kl_dev,
+                               float* recon_dev, void* stream);
+/* One training step of get_loss (:374-390): a train-mode forward, the Chamfer distance, losses_dev[3] = {loss,
+ * loss.cd, loss.kl} with loss = cd + kl_weight * sum(kl) / batch, and the backward pass into flat_grads_dev (same
+ * layout as the parameters, overwritten; the running statistics get 0).  The pass is kept for ds_shape_ae_get_knn. */
+DS_API int ds_shape_ae_train_step(ds_shape_ae* h, float* flat_params_dev, const float* points_dev, int32_t batch,
+                                  const float* eps_dev, float kl_weight, float* flat_grads_dev, float* losses_dev,
+                                  void* stream);
+/* The reference's chamfer_3DDist as a standalone op: for a [batch, n, 3] and b [batch, m, 3], dist1 [batch, n] is the
+ * squared distance from each point of a to its nearest point of b, idx1 its index (the first minimum in index order),
+ * and dist2 / idx2 the same from b to a.  The backward pass takes d(dist1), d(dist2) and writes grad_a [batch, n, 3]
+ * and / or grad_b [batch, m, 3] (either may be NULL) as gathers in a fixed order: bit-identical from run to run. */
+DS_API int ds_chamfer_forward(const float* a_dev, int32_t n, const float* b_dev, int32_t m, int32_t batch,
+                              float* dist1_dev, float* dist2_dev, int32_t* idx1_dev, int32_t* idx2_dev, void* stream);
+DS_API int ds_chamfer_backward(const float* a_dev, int32_t n, const float* b_dev, int32_t m, int32_t batch,
+                               const int32_t* idx1_dev, const int32_t* idx2_dev, const float* g1_dev,
+                               const float* g2_dev, float* grad_a_dev, float* grad_b_dev, void* stream);
+
 /* ---- introspection / debugging ------------------------------------------------------------ */
+/* The encoder's kNN (k = 16, the point itself included): x [batch, num_points, channels] fp32 -> idx [batch,
+ * num_points, 16] int32, ascending squared distance sum_c (x_i - x_j)^2 in fp32, ties broken by the lower index.
+ * channels in {3, 64, 128}, num_points >= 16. */
+DS_API int ds_knn(const float* x_dev, int32_t batch, int32_t num_points, int32_t channels, int32_t* idx_dev,
+                  void* stream);
+/* Parity aid: idx_dev [3, batch, num_points, 16] int32 (the xyz, 64-d and 128-d stages) replaces the shape
+ * auto-encoder's own kNN in every following forward / training step until it is set to NULL.  The pointer must stay
+ * valid and hold indices for the batch size of each call. */
+DS_API int ds_shape_ae_set_knn(ds_shape_ae* h, const int32_t* idx_dev);
+/* The three stages' kNN indices [3, batch, num_points, 16] of the last kept pass.  DS_ERR_INVALID when there is none. */
+DS_API int ds_shape_ae_get_knn(ds_shape_ae* h, int32_t* idx_dev, void* stream);
 /* Human-readable op list of the step program (works without a device when h == NULL: builds the plan
  * for `cfg` on the host only).  Returns bytes written (excluding NUL) or a negative status. */
 DS_API int ds_plan_describe(const ds_config* cfg, char* buf, int64_t buf_len);
