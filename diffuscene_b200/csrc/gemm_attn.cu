@@ -175,14 +175,22 @@ __device__ __forceinline__ void linattn_core(bf16* sbase, int h, bf16* out, int 
 #pragma unroll
     for (int np = 0; np < 2; ++np)
       at_ldsm_x4_t(b[np], k_a + uint32_t(((16 * kt + 8 * (mi & 1) + mr) * AT_LDS + 8 * (2 * np + (mi >> 1))) * 2));
-    // tokens >= NOBJ of this 16-token step are rows of the NEXT scene (or the zeroed tail): drop them from the v operand.
-    // A fragment of m16n8k16: a0 / a1 hold k = 2t, 2t + 1; a2 / a3 hold k = 2t + 8, 2t + 9
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt) {
+    // tokens >= NOBJ of this 16-token step are rows of the NEXT scene (possibly mid-softmax in another warp) or rows
+    // past M left by an earlier, larger batch: drop them from BOTH operands, since 0 * NaN = NaN would carry a
+    // non-finite neighbour into this scene.  A fragment of m16n8k16: a0 / a1 hold k = 2t, 2t + 1; a2 / a3 hold
+    // k = 2t + 8, 2t + 9.  B fragment: b0 holds k = 2t, 2t + 1, b1 holds k = 2t + 8, 2t + 9 (b[np][0|2] / b[np][1|3]).
+    {
       const int k0 = 16 * kt + 2 * t, k1 = k0 + 8;
       const uint32_t m0 = (k0 + 1 < NOBJ) ? 0xffffffffu : (k0 < NOBJ ? 0x0000ffffu : 0u);
       const uint32_t m1 = (k1 + 1 < NOBJ) ? 0xffffffffu : (k1 < NOBJ ? 0x0000ffffu : 0u);
-      a[mt][0] &= m0; a[mt][1] &= m0; a[mt][2] &= m1; a[mt][3] &= m1;
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt) {
+        a[mt][0] &= m0; a[mt][1] &= m0; a[mt][2] &= m1; a[mt][3] &= m1;
+      }
+#pragma unroll
+      for (int np = 0; np < 2; ++np) {
+        b[np][0] &= m0; b[np][2] &= m0; b[np][1] &= m1; b[np][3] &= m1;
+      }
     }
 #pragma unroll
     for (int mt = 0; mt < 2; ++mt)

@@ -88,3 +88,31 @@ def test_bf16_emulation_error_is_bounded(golden_dir):
     out = _run("bed62", no_reuse=False, bf16=True)
     err = (out - gold).abs()
     assert err.max() < 0.05 and err.mean() < 0.01, (err.max(), err.mean())
+
+
+def _reads(op):
+    """(buffer, first column, last column + 1) of every buffer slice an op reads."""
+    from oracle.plan_interp import OP_PACK
+    if op["kind"] == OP_PACK:
+        return []
+    r = [(s["buf"], s["col"], s["col"] + s["k"]) for s in (op["in0"], op["in1"]) if s["buf"] >= 0]
+    if op.get("res", -1) >= 0:
+        r.append((op["res"], 0, None))
+    return r
+
+
+@pytest.mark.parametrize("fuse", [0, 1, 4, 5])
+@pytest.mark.parametrize("name", ["bed62", "liv65", "text62", "arr5"])
+def test_no_reuse_plan_taps_are_op_inputs(name, fuse):
+    """In the program exported with no_reuse (the one the engine runs with taps on), no op reads a buffer that a
+    later op writes, and no op writes a buffer it reads.  So after one forward, the buffers an op read still hold
+    exactly what it read: the per-op GPU test evaluates each op from those taps."""
+    case = CASES[name]
+    spec = NetSpec.from_net_kwargs(case["net_kwargs"])
+    plan = capi.plan_export(capi.make_config(spec, case["N"], 1000, fuse_level=fuse), no_reuse=True)
+    ops = plan["ops"]
+    for i, op in enumerate(ops):
+        read = {b for b, _, _ in _reads(op)}
+        assert op["out"] not in read, op["name"]
+        for later in ops[i + 1:]:
+            assert later["out"] not in read, (op["name"], later["name"])
