@@ -50,6 +50,11 @@ class DsShapeAeConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("latent_dim", "num_points", "device")] + [("reserved", C.c_int32 * 5)]
 
 
+class DsTextEncConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("layers", "hidden", "heads", "intermediate", "vocab", "max_positions",
+                                         "type_vocab", "precision", "capacity", "device")] + [("reserved", C.c_int32 * 6)]
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -131,6 +136,12 @@ def load(rebuild: bool = False):
         "ds_knn": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, p]),
         "ds_chamfer_forward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p]),
         "ds_chamfer_backward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p, p, p]),
+        "ds_text_enc_create": (C.c_int, [C.POINTER(DsTextEncConfig), C.POINTER(H)]),
+        "ds_text_enc_destroy": (C.c_int, [H]),
+        "ds_text_enc_expected_weight_count": (C.c_int, [H]),
+        "ds_text_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+        "ds_text_enc_set_weights": (C.c_int, [H, p, p]),
+        "ds_text_enc_forward": (C.c_int, [H, p, p, C.c_int32, C.c_int32, p, p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -151,7 +162,9 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_shape_ae_create",
             "ds_shape_ae_destroy", "ds_shape_ae_expected_weight_count", "ds_shape_ae_expected_weight",
             "ds_shape_ae_forward", "ds_shape_ae_train_step", "ds_shape_ae_set_knn", "ds_shape_ae_get_knn", "ds_knn",
-            "ds_chamfer_forward", "ds_chamfer_backward"]
+            "ds_chamfer_forward", "ds_chamfer_backward", "ds_text_enc_create", "ds_text_enc_destroy",
+            "ds_text_enc_expected_weight_count", "ds_text_enc_expected_weight", "ds_text_enc_set_weights",
+            "ds_text_enc_forward"]
 
 
 class DsError(RuntimeError):

@@ -146,6 +146,20 @@ void launch_re_fold(const float* W, const float* bn, const RoomConvGeom& g, T* w
 void launch_re_fold_bwd(const float* dwp, const float* dbias, const float* W, const float* bn, const RoomConvGeom& g,
                         float* dW, float* dbn, cudaStream_t s);
 
+// ---- frozen BERT text encoder (text_encoder.cu): token rows [B * L, width] -------------------------------------
+// out = LayerNorm(word[ids[r]] + token_type[0] + position[r % L]) with weight g, bias b; NaN rows for ids outside
+// [0, vocab)
+template <typename TO>
+void launch_te_embed_ln(const int* ids, const float* word, const float* pos, const float* type0, const float* g,
+                        const float* b, TO* out, int M, int L, int H, int vocab, float eps, cudaStream_t s);
+template <typename TI, typename TO>
+void launch_te_layernorm(const TI* in, const float* g, const float* b, TO* out, int M, int H, float eps, cudaStream_t s);
+// masked self-attention, head dim 64, scale 1/8: qkv [B * L, 3H] -> out [B * L, H]; keys at or past lengths[b]
+// (clamped to [1, L]) get zero weight
+template <typename T>
+void launch_te_attention(const T* qkv, const int* lengths, T* out, int B, int L, int H, cudaStream_t s);
+template <typename T> void launch_te_convert(const float* in, T* out, int64_t n, cudaStream_t s);
+
 // ---- GEMMs: D[M,N] = act([A0 | A1][M, K0+K1] * W[N, K0+K1]^T + bias) (+ residual) -----------------
 struct GemmArgs {
   const void* a0; int lda0; int k0;

@@ -33,6 +33,7 @@ from ..parallel import allreduce_flat, allreduce_gradients
 from ..room_encoder import RoomEncoderFn, RoomMaskEncoder, trunk_specs
 from ..schedule import get_betas, make_tables
 from ..stats_logger import StatsLogger
+from ..text_encoder import BertTextEncoder
 from ..weights import NetSpec, seeded_tensor, unet1d_param_specs
 from .functional import DenoiserFn, room_trunk
 
@@ -519,14 +520,13 @@ class DiffusionSceneLayout_DDPM(nn.Module):
         if self.bertmodel is None:
             from transformers import BertModel, BertTokenizer
             self.tokenizer = BertTokenizer.from_pretrained("bert-base-cased")
-            bert = BertModel.from_pretrained("bert-base-cased").to(device).eval()
-            for p in bert.parameters():
-                p.requires_grad = False
-            object.__setattr__(self, "bertmodel", bert)          # frozen, kept out of _modules / state_dict
-        tok = self.tokenizer(text, return_tensors="pt", padding=True).to(device)
-        with torch.no_grad():
-            hid = self.bertmodel(**tok).last_hidden_state
-        return self.fc_text_f(hid)
+            bert = BertModel.from_pretrained("bert-base-cased").eval()      # on the CPU: only its weights are used
+            dev = torch.device(device)
+            enc = BertTextEncoder(bert, precision=self._precision,
+                                  device=dev.index if dev.index is not None else torch.cuda.current_device())
+            object.__setattr__(self, "bertmodel", enc)           # frozen, kept out of _modules / state_dict
+        tok = self.tokenizer(text, return_tensors="pt", padding=True)
+        return self.fc_text_f(self.bertmodel(**tok))
 
     # ---- training loss (reference :131-226) -------------------------------------------------------
     def _pack_target(self, sample_params):

@@ -353,6 +353,48 @@ DS_API int ds_chamfer_backward(const float* a_dev, int32_t n, const float* b_dev
                                const int32_t* idx1_dev, const int32_t* idx2_dev, const float* g1_dev,
                                const float* g2_dev, float* grad_a_dev, float* grad_b_dev, void* stream);
 
+/* ---- frozen BERT text encoder ------------------------------------------------------------------
+ * The forward pass of Hugging Face `BertModel` up to `last_hidden_state` (no pooler, no backward pass), which the
+ * text-conditioned networks run on each tokenized description: embeddings + LayerNorm, then `layers` post-LN blocks
+ * of masked self-attention (head dim 64, scale 1/8) and an erf-GELU feed-forward, LayerNorm eps 1e-12.  In bf16 mode
+ * the feed-forward GELU is the tanh form of the tensor-core GEMM epilogue.  A handle of its own, independent of
+ * ds_handle.
+ * Parameters are ONE flat fp32 device buffer in ds_text_enc_expected_weight() order: the `BertModel` state-dict names
+ * and sizes in state-dict order (embeddings.word_embeddings.weight, ..., encoder.layer.{i}.output.LayerNorm.bias),
+ * `pooler.*` left out.  ds_text_enc_set_weights copies and packs them, so the buffer may be released afterwards.
+ * Buffers for `capacity` tokens are allocated at creation; nothing is allocated inside a call.  `stream` is used as
+ * given. */
+typedef struct ds_text_enc ds_text_enc;
+typedef struct ds_text_enc_config {
+  int32_t layers;           /* num_hidden_layers, >= 1 (12 for bert-base-cased)                                  */
+  int32_t hidden;           /* hidden_size = 64 x heads, a multiple of 128 (768)                                */
+  int32_t heads;            /* num_attention_heads (12)                                                          */
+  int32_t intermediate;     /* intermediate_size, a multiple of 128 (3072)                                       */
+  int32_t vocab;            /* vocab_size (28996)                                                                */
+  int32_t max_positions;    /* max_position_embeddings: the longest sequence accepted (512)                     */
+  int32_t type_vocab;       /* type_vocab_size (2); only token type 0 is used                                    */
+  int32_t precision;        /* ds_precision: fp32 parity mode or bf16 tensor-core mode                          */
+  int32_t capacity;         /* tokens (batch x padded length) one forward may hold, 1 .. 4194240                 */
+  int32_t device;           /* CUDA device ordinal                                                               */
+  int32_t reserved[6];
+} ds_text_enc_config;
+/* DS_ERR_INVALID for any other geometry or capacity. */
+DS_API int ds_text_enc_create(const ds_text_enc_config* cfg, ds_text_enc** out);
+DS_API int ds_text_enc_destroy(ds_text_enc* h);
+DS_API int ds_text_enc_expected_weight_count(ds_text_enc* h);
+DS_API int ds_text_enc_expected_weight(ds_text_enc* h, int index, const char** name, int64_t* numel);
+/* Copies the flat parameters and packs the weight matrices (bf16 and a fused query/key/value matrix in bf16 mode),
+ * ordered on `stream`. */
+DS_API int ds_text_enc_set_weights(ds_text_enc* h, const float* flat_params_dev, void* stream);
+/* ids [batch, seq_len] int32 right-padded token ids, lengths [batch] int32 valid tokens per sequence -> out [batch,
+ * seq_len, hidden] fp32, device pointers.  Every position is computed, padding included: a padded query attends to
+ * its sequence's first lengths[b] keys like any other query.  Token type 0 throughout.  An id outside [0, vocab) gives
+ * a NaN row and reads nothing; lengths are clamped to [1, seq_len].  A sequence's output does not depend on the other
+ * sequences of the batch.  DS_ERR_STATE before ds_text_enc_set_weights; DS_ERR_INVALID for NULL pointers, seq_len
+ * above max_positions or batch x seq_len above the capacity. */
+DS_API int ds_text_enc_forward(ds_text_enc* h, const int32_t* ids_dev, const int32_t* lengths_dev, int32_t batch,
+                               int32_t seq_len, float* out_dev, void* stream);
+
 /* ---- introspection / debugging ------------------------------------------------------------ */
 /* The encoder's kNN (k = 16, the point itself included): x [batch, num_points, channels] fp32 -> idx [batch,
  * num_points, 16] int32, ascending squared distance sum_c (x_i - x_j)^2 in fp32, ties broken by the lower index.
