@@ -111,6 +111,8 @@ def load(rebuild: bool = False):
         "ds_adam_step": (C.c_int, [p, p, p, p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, p,
                                    C.c_float, p]),
         "ds_retrieve_objects": (C.c_int, [p, C.c_int32, p, p, C.c_int32, C.c_int32, p, p, p, C.c_int32, C.c_int32, p, p]),
+        "ds_scene_boxes": (C.c_int, [p, p, p, p, C.c_int32, p, p, C.c_int32, p, p, C.c_int32, p, p]),
+        "ds_scene_stats": (C.c_int, [p, p, p, p, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]),
         "ds_plan_describe": (C.c_int, [C.POINTER(DsConfig), C.c_char_p, C.c_int64]),
         "ds_plan_export_json": (C.c_int, [C.POINTER(DsConfig), C.c_int32, C.c_char_p, C.c_int64]),
         "ds_enable_taps": (C.c_int, [H, C.c_int32]),
@@ -164,7 +166,7 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_shape_ae_forward", "ds_shape_ae_train_step", "ds_shape_ae_set_knn", "ds_shape_ae_get_knn", "ds_knn",
             "ds_chamfer_forward", "ds_chamfer_backward", "ds_text_enc_create", "ds_text_enc_destroy",
             "ds_text_enc_expected_weight_count", "ds_text_enc_expected_weight", "ds_text_enc_set_weights",
-            "ds_text_enc_forward"]
+            "ds_text_enc_forward", "ds_scene_boxes", "ds_scene_stats"]
 
 
 class DsError(RuntimeError):

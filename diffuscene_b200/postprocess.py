@@ -74,11 +74,17 @@ class ObjectCatalog:
     grouped by class once (stable, so catalogue order inside a class -- the reference's tie-break -- is kept);
     `retrieve` answers a whole [B, N] batch of generated objects with ONE kernel launch (one warp per object) and
     returns indices into the ORIGINAL catalogue order (-1: class has no model).  Indices are bit-exact with the
-    reference's per-object numpy code (the kernel accumulates in numpy's float32 summation order)."""
+    reference's per-object numpy code (the kernel accumulates in numpy's float32 summation order).
+
+    For scene evaluation (diffuscene_b200.evaluate) two optional keyword arguments, both in original catalogue order:
+    `footprints`, the dict `evaluate.footprint_table` builds (one CSR table of xz hull polygons, raw half sizes and
+    raw AABBs, kept on the device; a model with an empty hull row is evaluated as its own box), and `model_ids` [M]
+    int, which stand in for the reference's model jids in the symmetry test (default: the catalogue index)."""
 
     MODES = {"objfeats_and_size": 0, "objfeats": 1, "box": 2}
+    FOOTPRINT_KEYS = ("hull_offsets", "hull_xz", "raw_half", "raw_aabb")
 
-    def __init__(self, labels, feats, sizes, n_classes=None, device="cuda"):
+    def __init__(self, labels, feats, sizes, n_classes=None, device="cuda", footprints=None, model_ids=None):
         import ctypes as C
         from . import capi
         self._C, self._capi = C, capi
@@ -95,6 +101,22 @@ class ObjectCatalog:
         self.class_start = start.to(dev)
         self.feats = None if feats is None else torch.as_tensor(feats, dtype=torch.float32)[order].contiguous().to(dev)
         self.sizes = None if sizes is None else torch.as_tensor(sizes, dtype=torch.float32)[order].contiguous().to(dev)
+        M = labels.numel()
+        ids = torch.arange(M) if model_ids is None else torch.as_tensor(model_ids, dtype=torch.int64).reshape(-1)
+        if ids.numel() != M:
+            raise ValueError("model_ids holds %d entries for %d catalogue models" % (ids.numel(), M))
+        self.model_ids = ids.to(dev)
+        self.footprints = None
+        if footprints is not None:
+            fp = {k: torch.as_tensor(footprints[k]) for k in self.FOOTPRINT_KEYS}
+            H = fp["hull_xz"].reshape(-1, 2).shape[0]
+            if fp["hull_offsets"].shape != (M + 1,) or fp["raw_half"].numel() != 3 * M or fp["raw_aabb"].numel() != 6 * M:
+                raise ValueError("footprint table does not describe %d models" % M)
+            self.footprints = {
+                "hull_offsets": fp["hull_offsets"].to(torch.int32).contiguous().to(dev),
+                "hull_xz": fp["hull_xz"].to(torch.float64).reshape(H, 2).contiguous().to(dev),
+                "raw_half": fp["raw_half"].to(torch.float64).reshape(M, 3).contiguous().to(dev),
+                "raw_aabb": fp["raw_aabb"].to(torch.float64).reshape(M, 6).contiguous().to(dev)}
 
     def retrieve(self, class_index, objfeats=None, sizes=None, mode="objfeats_and_size"):
         """class_index [...] int64, objfeats [..., F], sizes [..., 3] (world-space, i.e. after post_process_batch) ->

@@ -275,6 +275,40 @@ DS_API int ds_retrieve_objects(const int32_t* class_start_dev, int32_t n_classes
                                const int64_t* q_label_dev, const float* q_feat_dev, const float* q_size_dev,
                                int32_t num_queries, int32_t mode, int64_t* out_index_dev, void* stream);
 
+/* ---- post-processing: scene evaluation -------------------------------------------------------
+ * The statistics the reference writes with --compute_intersec (scripts/utils.py:560-745) for a whole batch of
+ * generated scenes.  Both calls are stateless; all pointers are device pointers.
+ *
+ * ds_scene_boxes: per object q of num_objects, the world-space axis-aligned bounds [x1, y1, z1, x2, y2, z2] (fp64)
+ * of its retrieved model placed as scene_synthesis/utils.py:114-163 places it: scaled by size / raw_half, centred on
+ * the scaled raw AABB, rotated about y by angle and translated.  translation [Q, 3], size [Q, 3] (half extents) and
+ * angle [Q] are fp32 world-space attributes.  model_index [Q] indexes the footprint table; -1 (or a NULL
+ * model_index, or a model whose hull row is empty) makes the object its own box: half sizes = size, centred.
+ * The footprint table of num_models models: hull_offsets [num_models + 1] int32 (row m of hull_xz is hull_offsets[m]
+ * .. hull_offsets[m + 1]), hull_xz [num_hull_vertices, 2] the raw xz convex-hull vertices, raw_half [num_models, 3]
+ * and raw_aabb [num_models, 6] (min xyz, max xyz of the raw vertices), fp64.  The x / z bounds are exact over the
+ * hull, y over the raw range.  DS_ERR_INVALID for NULL pointers, negative counts, hull offsets that are negative,
+ * decrease or pass num_hull_vertices, and a model index outside [-1, num_models); the last two are found on the
+ * device, so this call waits for `stream`.
+ *
+ * ds_scene_stats: one scene per row b of batch, over its kept objects (keep [batch, num_objects] uint8, NULL = all),
+ * num_objects <= 64: bounds [batch, num_objects, 6] fp64 as ds_scene_boxes writes them, class [batch, num_objects]
+ * int64, model_id [batch, num_objects] int64 (NULL: the symmetry test does not compare models).  Outputs per scene:
+ * the kept objects, the pairs n (n - 1) / 2, the fp32 IoU sum over pairs i < j in lexicographic order (the bounds
+ * rounded to fp32, each pair bit-equal to the reference's), the pairs with IoU > 0, the overlap ratio (fp32 from overlap and
+ * volume sums taken in fp64; 0 / 0 gives NaN) and the symmetric pairs (judge_if_symmetry on the fp64 bounds, equal class and model).  Scenes with 0 or
+ * 1 kept objects give (n, 1, 0, 0, 0) and 0, as the reference does.  pair_iou [batch, num_objects, num_objects]
+ * (optional) receives the IoU matrix by slot, 0 where a slot is not kept.  No atomics: a scene's outputs do not depend
+ * on the batch.  DS_ERR_INVALID for NULL required pointers, batch < 0 or num_objects outside [0, 64]. */
+DS_API int ds_scene_boxes(const float* translation_dev, const float* size_dev, const float* angle_dev,
+                          const int64_t* model_index_dev, int32_t num_objects, const int32_t* hull_offsets_dev,
+                          const double* hull_xz_dev, int32_t num_hull_vertices, const double* raw_half_dev,
+                          const double* raw_aabb_dev, int32_t num_models, double* bounds_dev, void* stream);
+DS_API int ds_scene_stats(const double* bounds_dev, const uint8_t* keep_dev, const int64_t* class_dev,
+                          const int64_t* model_id_dev, int32_t batch, int32_t num_objects, int32_t* num_objects_dev,
+                          int32_t* num_pairs_dev, float* iou_sum_dev, int32_t* insec_count_dev,
+                          float* overlap_ratio_dev, int32_t* num_symmetry_dev, float* pair_iou_dev, void* stream);
+
 /* ---- floor-plan encoder --------------------------------------------------------------------
  * Replaces the ResNet-18 trunk of the reference's room-mask feature extractor (scene_synthesis/networks/
  * feature_extractors.py:19-47 with FrozenBatchNorm2d, frozen_batchnorm.py): conv1 -> bn1 -> ReLU -> maxpool ->
