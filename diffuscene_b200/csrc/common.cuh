@@ -23,7 +23,7 @@ template <typename T> __device__ __forceinline__ float ldf(const T* p) { return 
 template <typename T> __device__ __forceinline__ void stf(T* p, float v) { ST<T>::st(p, v); }
 
 // ---- activations (exact forms: parity mode must match torch's erf-GELU / SiLU) ----
-enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_SILU = 2 };
+enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_SILU = 2, ACT_RELU = 3 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + __expf(-x)); }
@@ -31,6 +31,7 @@ __device__ __forceinline__ float silu_exact(float x) { return x / (1.0f + expf(-
 template <bool EXACT> __device__ __forceinline__ float apply_act(float x, int act) {
   if (act == ACT_GELU) return gelu_erf(x);
   if (act == ACT_SILU) return EXACT ? silu_exact(x) : silu(x);
+  if (act == ACT_RELU) return x < 0.f ? 0.f : x;      // NaN passes through, as torch.relu
   return x;
 }
 

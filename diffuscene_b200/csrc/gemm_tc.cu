@@ -253,6 +253,7 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
           y += chan[c + e];
           if (epi.act == ACT_GELU) y = gelu_tanh(y);
           else if (epi.act == ACT_SILU) y = silu_tanh(y);
+          else if (epi.act == ACT_RELU) y = y < 0.f ? 0.f : y;
         }
         v[e] = y;
       }

@@ -429,6 +429,61 @@ DS_API int ds_text_enc_set_weights(ds_text_enc* h, const float* flat_params_dev,
 DS_API int ds_text_enc_forward(ds_text_enc* h, const int32_t* ids_dev, const int32_t* lengths_dev, int32_t batch,
                                int32_t seq_len, float* out_dev, void* stream);
 
+/* ---- improved precision and recall of rendered scenes ------------------------------------------
+ * Feature extractor: torchvision `vgg16` as scripts/improved_precision_recall.py:159-163 (reference) uses it,
+ * `classifier[:4](features(x).view(-1, 7 * 7 * 512))`, i.e. the fc2 output before its ReLU, for images already
+ * normalised with the ImageNet mean / std.  No avgpool (the identity at 224 x 224).  bf16 mode runs the 13 3x3
+ * convolutions as implicit GEMMs on wgmma (NHWC bf16 activations, fp32 accumulation, bias + ReLU (+ 2x2 max-pool) in
+ * the epilogue) and fc1 / fc2 on the tensor-core GEMM; fp32 mode runs im2col and the exact SIMT GEMM.  The features
+ * are fp32 in both modes.
+ * Parameters are ONE flat fp32 device buffer in ds_vgg_expected_weight() order: the torchvision state-dict names and
+ * sizes in state-dict order, features.{0,2,5,7,10,12,14,17,19,21,24,26,28}.{weight,bias}, classifier.0.{weight,bias},
+ * classifier.3.{weight,bias} (classifier.6, which the feature never reaches, left out).  ds_vgg_set_weights packs them,
+ * so the buffer may be released afterwards.  A handle of its own, independent of ds_handle. */
+typedef struct ds_vgg ds_vgg;
+typedef struct ds_vgg_config {
+  int32_t precision;        /* ds_precision: fp32 parity mode or bf16 tensor-core mode                          */
+  int32_t capacity;         /* images one internal pass holds, 1 .. 256; larger batches run in passes of this size */
+  int32_t device;           /* CUDA device ordinal                                                               */
+  int32_t reserved[5];
+} ds_vgg_config;
+#define DS_VGG_FEATURES 4096
+DS_API int ds_vgg_create(const ds_vgg_config* cfg, ds_vgg** out);
+DS_API int ds_vgg_destroy(ds_vgg* h);
+DS_API int ds_vgg_expected_weight_count(ds_vgg* h);
+DS_API int ds_vgg_expected_weight(ds_vgg* h, int index, const char** name, int64_t* numel);
+/* DS_ERR_INVALID for NULL pointers or a parameter count other than the sum of the expected sizes. */
+DS_API int ds_vgg_set_weights(ds_vgg* h, const float* flat_params_dev, int64_t count, void* stream);
+/* images [batch, 3, height, width] fp32 NCHW, normalised -> features [batch, 4096] fp32, device pointers.  Images
+ * that are not 224 x 224 are resized with the pixel choice of F.interpolate(size=(224, 224)) in its default nearest
+ * mode (src = min(floor(dst * (float)in / 224), in - 1), the scale in fp32), as extract_features does
+ * (improved_precision_recall.py:152-156).  An image's features do not depend on the other images of the batch.
+ * DS_ERR_STATE before ds_vgg_set_weights; DS_ERR_INVALID for NULL pointers, batch < 0 or a side outside [1, 4096]. */
+DS_API int ds_vgg_features(ds_vgg* h, const float* images_dev, int32_t batch, int32_t height, int32_t width,
+                           float* features_dev, void* stream);
+
+/* Manifold metrics (improved_precision_recall.py:196-256) on fp64 features [rows, d] (row-major, any d >= 1), without
+ * an N x N matrix: distances are sqrt(max(0, (|x|^2 - 2 x.y) + |y|^2)) in fp64 on the fp64 tensor cores, and
+ * `clamped_dev` (int64 on the device, may be NULL) receives how many squared distances were negative and set to 0,
+ * as the reference prints.  Stateless; scratch is allocated on `stream`. */
+#define DS_MANIFOLD_MAX_K 16
+/* out [n, m] = distances of x [n, d] to y [m, d] (for small inputs and tests). */
+DS_API int ds_manifold_distances(const double* x_dev, int32_t n, const double* y_dev, int32_t m, int32_t d,
+                                 double* out_dev, int64_t* clamped_dev, void* stream);
+/* radii [n]: radius i is the (k+1)-th smallest distance of row i of x's self-distance matrix, the ~0 distance to
+ * itself counted (distances2radii).  DS_ERR_INVALID for NULL pointers, k outside [1, DS_MANIFOLD_MAX_K], n <= k or
+ * d < 1. */
+DS_API int ds_manifold_radii(const double* x_dev, int32_t n, int32_t d, int32_t k, double* radii_dev,
+                             int64_t* clamped_dev, void* stream);
+/* One pass over reference x subject pairs (compute_metric and realism, strict <):
+ *   subj_covered [n_subj] uint8: 1 when some reference i has dist(ref_i, subj_j) < ref_radii[i] (precision flags)
+ *   ref_covered  [n_ref]  uint8: 1 when some subject j has dist(ref_i, subj_j) < subj_radii[j] (recall flags)
+ *   realism      [n_subj] fp64:  max_i ref_radii[i] / (dist(ref_i, subj_j) + 1e-6)
+ * Each output may be NULL; ref_covered needs subj_radii.  DS_ERR_INVALID for NULL required pointers or a count < 1. */
+DS_API int ds_manifold_cover(const double* ref_dev, const double* ref_radii_dev, int32_t n_ref, const double* subj_dev,
+                             const double* subj_radii_dev, int32_t n_subj, int32_t d, uint8_t* subj_covered_dev,
+                             uint8_t* ref_covered_dev, double* realism_dev, int64_t* clamped_dev, void* stream);
+
 /* ---- introspection / debugging ------------------------------------------------------------ */
 /* The encoder's kNN (k = 16, the point itself included): x [batch, num_points, channels] fp32 -> idx [batch,
  * num_points, 16] int32, ascending squared distance sum_c (x_i - x_j)^2 in fp32, ties broken by the lower index.
@@ -458,6 +513,14 @@ DS_API int64_t ds_graph_build_count(ds_handle* h);
 /* Per-op device time of one forward (CUDA events around each op; profiling aid, not a bench number).
  * Writes up to `cap` entries of (name, microseconds). Returns op count. */
 DS_API int ds_profile_ops(ds_handle* h, int32_t batch, char* names_buf, int64_t names_len, float* usec, int32_t cap);
+/* One bf16 VGG16 convolution alone, for unit tests: x [batch, height, width, cin] fp32 NHWC, rounded to bf16 ->
+ * relu(conv3x3(x, W, b), pad 1) (-> 2 x 2 max-pool when pool != 0) [batch, height (/ 2), width (/ 2), cout] fp32,
+ * computed by the kernel ds_vgg_features runs (W [cout, cin, 3, 3] fp32, rounded to bf16 when packed; b [cout] fp32).
+ * cin is 3 (the first layer's im2col path) or a multiple of 64; cout is 64 or a multiple of 128; pooled sides are
+ * even.  Synchronises `stream`. */
+DS_API int ds_vgg_test_conv(const float* in_dev, int32_t batch, int32_t height, int32_t width, int32_t cin,
+                            int32_t cout, int32_t pool, const float* weight_dev, const float* bias_dev, float* out_dev,
+                            void* stream);
 /* Standalone GEMM for unit tests: D[M,N] = A[M,K] * W[N,K]^T (+bias), bf16 in / bf16 out via the selected
  * backend. Device pointers. */
 DS_API int ds_test_gemm_bf16(int backend, const void* a_dev, const void* w_dev, const float* bias_dev, void* d_dev,
