@@ -11,15 +11,18 @@
 //   wgmma       warpgroup g multiplies rows 64 g .. 64 g + 63 of the A tile with the whole W tile:
 //               wgmma.mma_async m64n128k16 x 4 per k-block, accumulator in 64 registers per thread.
 //               Two resident CTAs per SM let one CTA's epilogue overlap the other's MMAs.
-//   epilogue    from the accumulator registers; bf16 results are staged in the drained ring and written out as
-//               whole 256-byte rows.  Three forms:
+//   epilogue    from the accumulator registers; results are staged in the drained ring (bf16, or fp32 when a
+//               residual follows) and written out as whole 256-byte rows, the residual added in that row pass
+//               from 16-byte loads of whole rows.  Three forms:
 //                 plain  bias / GELU|SiLU / residual -> bf16
 //                 d32    split-K partial sums added to an fp32 output with atomics (weight-gradient GEMMs)
 //                 GN     the whole `Block` of the reference (denoise_net.py:160-176) after the conv:
 //                        bias -> GroupNorm(8) statistics per (scene, group) reduced across the rows of a
 //                        scene through shared memory -> affine -> FiLM -> SiLU (-> + residual).  M tiles
 //                        are whole scenes (120 of 128 rows for N=12, 126 for N=21), N tiles are 2 whole
-//                        groups of 64 channels, so the statistics never leave the CTA.
+//                        groups of 64 channels, so the statistics never leave the CTA.  The affine
+//                        coefficients per (scene, column) and the tile's FiLM rows are tabled in the ring
+//                        once, so the element loop reads two 16-byte entries per column pair.
 // Both operands are K-major (activations [rows, K], weights [N, K] exactly as PyTorch stores them), so no
 // transposes exist anywhere in the data path.  A "virtual concat" [A0|A1] (the U-Net skip connections,
 // denoise_net.py:562,566,573) is served by switching tensor maps inside the k loop.
@@ -44,10 +47,18 @@ static constexpr int PART_OFF = CHAN_OFF + 3 * BN * 4;
 static constexpr int STAT_OFF = PART_OFF + BM * 2 * 8;
 static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAT_OFF + BM * 2 * 8;
 static_assert(2 * (SMEM_BYTES + 1024) <= 233472, "two CTAs per SM");
-// bf16 output tile staged in the drained ring before it is written out; the row pitch of 136 elements (68 words) puts
-// the 8 rows one fragment store touches on distinct banks
+// output tile staged in the drained ring before it is written out, bf16 or (launches with a residual) fp32.  The row
+// pitch of 136 elements puts the 8 rows one fragment store touches on distinct banks: 68 words for bf16 (one
+// wavefront), 136 words for fp32 (rows 4 apart share banks: two wavefronts, the least for 256 bytes)
 static constexpr int STG_PITCH = BN + 8;
-static_assert(BM * STG_PITCH * 2 <= STAGES * STAGE_BYTES, "staging tile fits in the ring");
+static constexpr int STG16_BYTES = BM * STG_PITCH * 2;
+static constexpr int STG32_BYTES = BM * STG_PITCH * 4;
+// GN epilogue tables behind the staging tile, one row of BN / 2 float4 per scene of the tile (GroupNorm affine) and
+// per FiLM row.  At most GN_MAX_SPT scenes per tile (>= 12 objects per scene), so the affine table always fits; the
+// FiLM table is used where it fits as well and read from global memory otherwise
+static constexpr int TBL_ROW_BYTES = BN / 2 * 16;
+static constexpr int GN_MAX_SPT = 10;
+static_assert(STG32_BYTES + 2 * GN_MAX_SPT * TBL_ROW_BYTES <= STAGES * STAGE_BYTES, "tables fit in the ring");
 
 struct TcEpi {
   const float* bias;
@@ -172,7 +183,48 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
     return;
   }
 
+  // the output tile is staged in the drained ring: fp32 when a residual is added in the row pass, else bf16
+  const bool stage32 = epi.res != nullptr;
+  const int tbl_off = stage32 ? STG32_BYTES : STG16_BYTES;
+  // GN: per (scene of the tile, column pair) float4 (a0, a1, b0, b1) of y = a x + b (GroupNorm affine with the conv
+  // bias folded in), then the FiLM rows of the tile as float4 (scale0 + 1, scale1 + 1, shift0, shift1) per column
+  // pair: one row per scene (time) or per object (shared context).  Both tables sit behind the staging tile.
+  float4* const ab_tab = reinterpret_cast<float4*>(base_ptr + tbl_off);
+  float4* film_tab = nullptr;
+  const float* film_row0 = nullptr;        // FiLM table rows are read from here on (column n0)
+  int film_rows = 0, film_items = 0;
+  int spt = 0;
   if constexpr (GN) {
+    spt = epi.tile_rows / epi.n_obj;
+    const int mode = epi.film.mode;
+    film_rows = mode == FILM_TIME ? min(spt, (epi.M - m0) / epi.n_obj) : mode == FILM_OBJECT ? epi.n_obj : 0;
+    if (film_rows && tbl_off + (spt + film_rows) * TBL_ROW_BYTES <= STAGES * STAGE_BYTES) {
+      film_tab = ab_tab + spt * (BN / 2);
+      film_row0 = epi.film.base + n0;
+      film_items = film_rows * (BN / 4);
+    }
+    // item i = (table row i / 32, columns 4 (i % 32) .. + 3): one float4 of scales and one of shifts
+    auto film_src = [&](int i) {
+      const int row = i / (BN / 4);
+      const int64_t r = mode == FILM_TIME ? (int64_t)__ldg(epi.film.t + m0 / epi.n_obj + row) : row;
+      return film_row0 + r * epi.film.row_stride + 4 * (i % (BN / 4));
+    };
+    float4 fs[2], fh[2];                   // the first two items of each thread, loaded before the barrier
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      const int i = tid + k * TC_THREADS;
+      if (i < film_items) {
+        const float* src = film_src(i);
+        fs[k] = __ldg(reinterpret_cast<const float4*>(src));
+        fh[k] = __ldg(reinterpret_cast<const float4*>(src + epi.C));
+      }
+    }
+    auto film_put = [&](int i, float4 s, float4 h) {
+      float4* dst = film_tab + (i / (BN / 4)) * (BN / 2) + 2 * (i % (BN / 4));
+      dst[0] = make_float4(s.x + 1.0f, s.y + 1.0f, h.x, h.y);
+      dst[1] = make_float4(s.z + 1.0f, s.w + 1.0f, h.z, h.w);
+    };
+
     // per-row partial (sum, sum of squares) of the two 64-channel groups of the tile: 16 values per thread,
     // then across the 4 threads of a quad that share the row
 #pragma unroll
@@ -196,8 +248,14 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
         if ((lane & 3) == 0) part[(r0 + 8 * h) * 2 + g] = make_float2(s, ss);
       }
     }
-    __syncthreads();
-    const int spt = epi.tile_rows / epi.n_obj;
+    __syncthreads();        // partials complete; every MMA of the CTA is done, so the ring is free
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+      if (tid + k * TC_THREADS < film_items) film_put(tid + k * TC_THREADS, fs[k], fh[k]);
+    for (int i = tid + 2 * TC_THREADS; i < film_items; i += TC_THREADS) {
+      const float* src = film_src(i);
+      film_put(i, __ldg(reinterpret_cast<const float4*>(src)), __ldg(reinterpret_cast<const float4*>(src + epi.C)));
+    }
     if (tid < spt * 2) {
       const int sc = tid >> 1, g = tid & 1;
       float s = 0.f, ss = 0.f;
@@ -212,68 +270,118 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tm_a0, const __grid_constant__ CUt
       stat[tid] = make_float2(mean, rsqrtf(var + 1e-5f));
     }
     __syncthreads();
-  } else {
-    __syncthreads();        // the other warpgroup's MMAs may still read the ring the tile is staged in
+    for (int i = tid; i < spt * (BN / 2); i += TC_THREADS) {
+      const int sc = i / (BN / 2), c = 2 * (i % (BN / 2));
+      const float2 st = stat[sc * 2 + c / GN_GROUP];
+      const float a0 = st.y * chan[BN + c], a1 = st.y * chan[BN + c + 1];
+      ab_tab[i] = make_float4(a0, a1, fmaf(chan[c] - st.x, a0, chan[2 * BN + c]),
+                              fmaf(chan[c + 1] - st.x, a1, chan[2 * BN + c + 1]));
+    }
   }
+  __syncthreads();        // GN: tables complete; plain: the other warpgroup's MMAs may still read the ring
 
-  bf16* const stg = reinterpret_cast<bf16*>(base_ptr);      // [BM][STG_PITCH]
+  float* const stg32 = reinterpret_cast<float*>(base_ptr);   // [BM][STG_PITCH] fp32 (launches with a residual)
+  bf16* const stg = reinterpret_cast<bf16*>(base_ptr);       // [BM][STG_PITCH] bf16
+  bool live[2];
+  int sc[2] = {0, 0}, fkey[2] = {0, 0};
+  const float* frow[2] = {nullptr, nullptr};   // GN without a FiLM table: this token's row [scale(C) | shift(C)] at n0
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int rt = r0 + 8 * h, m = m0 + rt;
-    if (rt >= epi.tile_rows || m >= epi.M) continue;
-    bf16* sp = stg + rt * STG_PITCH + cq;
-    const bf16* rp = epi.res ? epi.res + (int64_t)m * epi.ldres + n0 + cq : nullptr;
-    int sc = 0;
-    const float* frow = nullptr;         // FiLM row of this token: [scale(C) | shift(C)], already at column n0
+    live[h] = rt < epi.tile_rows && m < epi.M;
     if constexpr (GN) {
-      sc = rt / epi.n_obj;
-      if (epi.film.mode == FILM_TIME)
-        frow = epi.film.base + (int64_t)__ldg(epi.film.t + m / epi.n_obj) * epi.film.row_stride;
-      else if (epi.film.mode == FILM_OBJECT)
-        frow = epi.film.base + (int64_t)(m % epi.n_obj) * epi.film.row_stride;
-      else if (epi.film.mode == FILM_TOKEN)
-        frow = epi.film.base + (int64_t)m * epi.film.row_stride;
-      if (frow) frow += n0;
-    }
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int c = 8 * j + cq;
-      float v[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float y = acc[4 * j + 2 * h + e];
-        if constexpr (GN) {
-          const float2 st = stat[sc * 2 + (c >> 6)];
-          const float a = st.y * chan[BN + c + e];
-          const float b = fmaf(chan[c + e] - st.x, a, chan[2 * BN + c + e]);
-          y = fmaf(y, a, b);
-          if (frow) y = fmaf(y, __ldg(frow + c + e) + 1.0f, __ldg(frow + epi.C + c + e));
-          y = silu_tanh(y);
-        } else {
-          y += chan[c + e];
-          if (epi.act == ACT_GELU) y = gelu_tanh(y);
-          else if (epi.act == ACT_SILU) y = silu_tanh(y);
-          else if (epi.act == ACT_RELU) y = y < 0.f ? 0.f : y;
-        }
-        v[e] = y;
+      sc[h] = rt / epi.n_obj;
+      fkey[h] = epi.film.mode == FILM_TIME ? sc[h] : rt % epi.n_obj;
+      if (!film_tab && live[h]) {
+        if (epi.film.mode == FILM_TIME)
+          frow[h] = epi.film.base + (int64_t)__ldg(epi.film.t + m / epi.n_obj) * epi.film.row_stride + n0;
+        else if (epi.film.mode == FILM_OBJECT)
+          frow[h] = epi.film.base + (int64_t)(m % epi.n_obj) * epi.film.row_stride + n0;
+        else if (epi.film.mode == FILM_TOKEN)
+          frow[h] = epi.film.base + (int64_t)m * epi.film.row_stride + n0;
       }
-      if (rp) {
-        // plain (coherent) load, not __ldg: the backward GEMMs accumulate in place (res == d)
-        const float2 r2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(rp + 8 * j));
-        v[0] += r2.x;
-        v[1] += r2.y;
-      }
-      *reinterpret_cast<__nv_bfloat162*>(sp + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
     }
   }
-  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int c = 8 * j + cq, cp = 4 * j + (lane & 3);      // column, column pair
+    const float2 bias = *reinterpret_cast<const float2*>(chan + c);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!live[h]) continue;
+      float y0 = acc[4 * j + 2 * h], y1 = acc[4 * j + 2 * h + 1];
+      if constexpr (GN) {
+        const float4 ab = ab_tab[sc[h] * (BN / 2) + cp];
+        y0 = fmaf(y0, ab.x, ab.z);
+        y1 = fmaf(y1, ab.y, ab.w);
+        if (film_tab) {
+          const float4 f = film_tab[fkey[h] * (BN / 2) + cp];
+          y0 = fmaf(y0, f.x, f.z);
+          y1 = fmaf(y1, f.y, f.w);
+        } else if (frow[h]) {
+          const float2 s = __ldg(reinterpret_cast<const float2*>(frow[h] + c));
+          const float2 t = __ldg(reinterpret_cast<const float2*>(frow[h] + epi.C + c));
+          y0 = fmaf(y0, s.x + 1.0f, t.x);
+          y1 = fmaf(y1, s.y + 1.0f, t.y);
+        }
+        y0 = silu_tanh(y0);
+        y1 = silu_tanh(y1);
+      } else {
+        y0 += bias.x;
+        y1 += bias.y;
+        if (epi.act == ACT_GELU) { y0 = gelu_tanh(y0); y1 = gelu_tanh(y1); }
+        else if (epi.act == ACT_SILU) { y0 = silu_tanh(y0); y1 = silu_tanh(y1); }
+        else if (epi.act == ACT_RELU) { y0 = y0 < 0.f ? 0.f : y0; y1 = y1 < 0.f ? 0.f : y1; }
+      }
+      const int rt = r0 + 8 * h;
+      if (stage32) *reinterpret_cast<float2*>(stg32 + rt * STG_PITCH + c) = make_float2(y0, y1);
+      else *reinterpret_cast<__nv_bfloat162*>(stg + rt * STG_PITCH + c) = __floats2bfloat162_rn(y0, y1);
+    }
+  }
+
   // whole output rows: 16 threads x 16 bytes per 256-byte row, instead of the fragment layout's 16 bytes per row and
   // store instruction
-  for (int idx = tid; idx < BM * (BN / 8); idx += TC_THREADS) {
-    const int rt = idx / (BN / 8), c = (idx % (BN / 8)) * 8, m = m0 + rt;
-    if (rt < epi.tile_rows && m < epi.M)
-      *reinterpret_cast<uint4*>(epi.d + (int64_t)m * epi.ldd + n0 + c) =
-          *reinterpret_cast<const uint4*>(stg + rt * STG_PITCH + c);
+  constexpr int ROW_ITERS = BM * (BN / 8) / TC_THREADS;
+  if (stage32) {
+    // the residual is added here, read as whole rows: every load is issued before the first store (a thread reads
+    // its 16 bytes before it writes them, so accumulating in place, res == d, stays correct) and overlaps the barrier
+    uint4 rv[ROW_ITERS];
+#pragma unroll
+    for (int it = 0; it < ROW_ITERS; ++it) {
+      const int idx = tid + it * TC_THREADS, rt = idx / (BN / 8), m = m0 + rt;
+      if (rt < epi.tile_rows && m < epi.M)       // plain (coherent) load, not __ldg: res may be d
+        rv[it] = *reinterpret_cast<const uint4*>(epi.res + (int64_t)m * epi.ldres + n0 + (idx % (BN / 8)) * 8);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < ROW_ITERS; ++it) {
+      const int idx = tid + it * TC_THREADS, rt = idx / (BN / 8), q = idx % (BN / 8), m = m0 + rt;
+      if (rt >= epi.tile_rows || m >= epi.M) continue;
+      // the two halves in an order that gives the 8 threads of a quarter warp 8 distinct 16-byte bank groups
+      const float* sp = stg32 + rt * STG_PITCH + 8 * q;
+      const int sw = 4 * ((q >> 2) & 1);
+      const float4 u = *reinterpret_cast<const float4*>(sp + sw), w = *reinterpret_cast<const float4*>(sp + (4 - sw));
+      const float4 lo = sw ? w : u, hi = sw ? u : w;
+      const __nv_bfloat162* r2 = reinterpret_cast<const __nv_bfloat162*>(&rv[it]);
+      const float2 ra = __bfloat1622float2(r2[0]), rb = __bfloat1622float2(r2[1]);
+      const float2 rc = __bfloat1622float2(r2[2]), rd = __bfloat1622float2(r2[3]);
+      uint4 o;
+      __nv_bfloat162* o2 = reinterpret_cast<__nv_bfloat162*>(&o);
+      o2[0] = __floats2bfloat162_rn(lo.x + ra.x, lo.y + ra.y);
+      o2[1] = __floats2bfloat162_rn(lo.z + rb.x, lo.w + rb.y);
+      o2[2] = __floats2bfloat162_rn(hi.x + rc.x, hi.y + rc.y);
+      o2[3] = __floats2bfloat162_rn(hi.z + rd.x, hi.w + rd.y);
+      *reinterpret_cast<uint4*>(epi.d + (int64_t)m * epi.ldd + n0 + 8 * q) = o;
+    }
+  } else {
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < ROW_ITERS; ++it) {
+      const int idx = tid + it * TC_THREADS, rt = idx / (BN / 8), c = (idx % (BN / 8)) * 8, m = m0 + rt;
+      if (rt < epi.tile_rows && m < epi.M)
+        *reinterpret_cast<uint4*>(epi.d + (int64_t)m * epi.ldd + n0 + c) =
+            *reinterpret_cast<const uint4*>(stg + rt * STG_PITCH + c);
+    }
   }
 }
 
@@ -353,9 +461,9 @@ TcGemmPlan* tc_plan_create(const GemmArgs& g, int rows_capacity, char* err, int 
     return nullptr;
   }
   const bool gn = g.gn != 0;
-  if (gn && (g.N != 8 * GN_GROUP || g.n_obj < 1 || g.n_obj > BM || !g.gamma || !g.beta)) {
-    if (err) snprintf(err, err_len, "fused GroupNorm epilogue needs N == %d (8 groups of %d), 1 <= n_obj <= %d, gamma/beta",
-                      8 * GN_GROUP, GN_GROUP, BM);
+  if (gn && (g.N != 8 * GN_GROUP || g.n_obj < 1 || g.n_obj > BM || BM / g.n_obj > GN_MAX_SPT || !g.gamma || !g.beta)) {
+    if (err) snprintf(err, err_len, "fused GroupNorm epilogue needs N == %d (8 groups of %d), %d <= n_obj <= %d, gamma/beta",
+                      8 * GN_GROUP, GN_GROUP, BM / (GN_MAX_SPT + 1) + 1, BM);
     return nullptr;
   }
   TcGemmPlan* p = new TcGemmPlan();
