@@ -16,6 +16,10 @@ DS_PREC_FP32, DS_PREC_BF16 = 0, 1
 DS_GEMM_AUTO, DS_GEMM_SIMT, DS_GEMM_TCGEN05 = 0, 1, 2
 DS_MEAN_EPS, DS_MEAN_X0, DS_MEAN_V = 0, 1, 2
 MEAN_TYPES = {"eps": DS_MEAN_EPS, "x0": DS_MEAN_X0, "v": DS_MEAN_V}
+DS_TRAIN_ACT, DS_TRAIN_GRAD, DS_TRAIN_DW, DS_TRAIN_DVEC, DS_TRAIN_COND = range(5)
+TRAIN_COND = {n: i for i, n in enumerate((
+    "emb", "z1", "h1", "temb", "st", "film", "dfilm", "dtemb", "dh1", "dst", "ctx_act", "ctx_film", "dctx_film",
+    "dctx_act", "xkv", "xctx", "x_t"))}      # DS_TRAIN_COND indices (include/diffuscene_b200.h)
 
 
 class DsConfig(C.Structure):
@@ -111,6 +115,7 @@ def load(rebuild: bool = False):
                                           p, p, p, C.c_int32, p, C.c_int32, p]),
         "ds_train_set_buckets": (C.c_int, [H, p, C.c_int32, p]),
         "ds_train_phase_ms": (C.c_int, [H, p]),
+        "ds_train_read": (C.c_int, [H, C.c_int32, C.c_int32, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), p]),
         "ds_sumsq": (C.c_int, [p, C.c_int64, p, p]),
         "ds_adam_step": (C.c_int, [p, p, p, p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, p,
                                    C.c_float, p]),
@@ -172,7 +177,7 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_set_context",
             "ds_set_context_cross", "ds_denoise_forward", "ds_denoise_forward_host", "ds_sample_loop",
             "ds_sample_loop_host", "ds_traj_count", "ds_p_sample_step", "ds_q_sample", "ds_p_losses", "ds_retrieve_objects",
-            "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_sumsq", "ds_adam_step",
+            "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_train_read", "ds_sumsq", "ds_adam_step",
             "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
             "ds_test_gemm_bf16", "ds_room_enc_create", "ds_room_enc_destroy", "ds_room_enc_expected_weight_count",
             "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_shape_ae_create",

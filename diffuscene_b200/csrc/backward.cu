@@ -801,26 +801,25 @@ __global__ void __launch_bounds__(128) k_p_losses_bwd(const float* __restrict__ 
   __shared__ float s_nvalid;
   const float per_scene = grad_scale / float(B);      // loss = mean over the batch
   // ---- MSE part: slice means over (N, slice width), weights as in the reference's branches
+  auto mse_grad = [&](int o, int ch) {
+    const int64_t xi = ((int64_t)b * N + o) * d + ch;
+    float target;
+    if (a.mean_type == DS_MEAN_EPS) target = noise[xi];
+    else if (a.mean_type == DS_MEAN_X0) target = x0[xi];
+    else target = sa * noise[xi] - s1 * x0[xi];
+    const float diff = ldf(out + ((int64_t)b * N + o) * ld + ch) - target;
+    float wsl;      // 1 / (elements of the mean this channel belongs to), 0 if its term is not in the loss
+    if (!a.loss_separate) wsl = 1.0f / float(N * d);
+    else if (a.arrange) wsl = 1.0f / float(N * (ch < a.trans ? a.trans : d - a.trans));
+    else if (ch < bb) wsl = 1.0f / float(N * bb);
+    else if (ch < bb + a.cls) wsl = 1.0f / float(N * a.cls);
+    else if (ch < bb + a.cls + a.objn) wsl = 1.0f / float(N * a.objn);
+    else wsl = 1.0f / float(N * a.feat);
+    return 2.0f * diff * wsl * lw * per_scene;
+  };
   for (int i = tid; i < N * dpad; i += blockDim.x) {
     const int o = i / dpad, ch = i % dpad;
-    float g = 0.f;
-    if (ch < d) {
-      const int64_t xi = ((int64_t)b * N + o) * d + ch;
-      float target;
-      if (a.mean_type == DS_MEAN_EPS) target = noise[xi];
-      else if (a.mean_type == DS_MEAN_X0) target = x0[xi];
-      else target = sa * noise[xi] - s1 * x0[xi];
-      const float diff = ldf(out + ((int64_t)b * N + o) * ld + ch) - target;
-      float wsl;      // 1 / (elements of the mean this channel belongs to), 0 if its term is not in the loss
-      if (!a.loss_separate) wsl = 1.0f / float(N * d);
-      else if (a.arrange) wsl = 1.0f / float(N * (ch < a.trans ? a.trans : d - a.trans));
-      else if (ch < bb) wsl = 1.0f / float(N * bb);
-      else if (ch < bb + a.cls) wsl = 1.0f / float(N * a.cls);
-      else if (ch < bb + a.cls + a.objn) wsl = 1.0f / float(N * a.objn);
-      else wsl = 1.0f / float(N * a.feat);
-      g = 2.0f * diff * wsl * lw * per_scene;
-    }
-    stf(dout + ((int64_t)b * N + o) * ldd + ch, g);
+    stf(dout + ((int64_t)b * N + o) * ldd + ch, ch < d ? mse_grad(o, ch) : 0.f);
   }
   if (!a.loss_iou) return;
   __syncthreads();
@@ -911,8 +910,8 @@ __global__ void __launch_bounds__(128) k_p_losses_bwd(const float* __restrict__ 
     else g = (dcorn[o][k] - dcorn[o][k - 3]) * 0.5f * (a.bounds[9 + (k - 3)] - a.bounds[6 + (k - 3)]);       // d/d size: hi - lo
     g *= pass[o][k] * ao;
     const int ch = k < 3 ? k : a.trans + (k - 3);
-    T* p = dout + ((int64_t)b * N + o) * ldd + ch;
-    stf(p, ldf(p) + g);
+    // the MSE term again in fp32 rather than read back, so that a bf16 gradient is rounded once
+    stf(dout + ((int64_t)b * N + o) * ldd + ch, mse_grad(o, ch) + g);
   }
 }
 template <typename T>

@@ -165,6 +165,7 @@ struct TrainState {
   std::vector<cudaEvent_t> bucket_events;
   cudaEvent_t ev[7] = {nullptr};      // phase boundaries of the last step (ds_train_phase_ms)
   bool ev_valid = false;
+  int last_B = 0, last_L = 0, last_ctx_rows = 0;      // shape of the last step with gradients (ds_train_read)
 };
 
 void train_state_destroy(TrainState* t) {
@@ -862,6 +863,9 @@ static int train_step_t(ds_handle* h, const float* flat, const float* x0, const 
   advance_buckets();
   cudaEventRecord(t->ev[6], s);
   t->ev_valid = true;
+  t->last_B = B;
+  t->last_L = cross ? L : 0;
+  t->last_ctx_rows = ctx_rows;
   CK(cudaGetLastError());
   return 0;
 }
@@ -948,6 +952,83 @@ extern "C" int ds_train_phase_ms(ds_handle* h, float* out6) {
   if (!h || !out6 || !h->train || !h->train->ev_valid) return fail(DS_ERR_STATE, "no completed training step with gradients");
   CK(cudaEventSynchronize(h->train->ev[6]));
   for (int i = 0; i < 6; ++i) CK(cudaEventElapsedTime(out6 + i, h->train->ev[i], h->train->ev[i + 1]));
+  return 0;
+}
+
+namespace {
+__global__ void k_widen_bf16(const ds::bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = __bfloat162float(in[i]);
+}
+}  // namespace
+
+extern "C" int ds_train_read(ds_handle* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity, int32_t* rows,
+                             int32_t* width, void* stream) {
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  TrainState* t = h->train;
+  if (!t || !t->ev_valid) return fail(DS_ERR_STATE, "no completed training step with gradients");
+  const Plan& P = t->plan;
+  const int B = t->last_B, C = P.C, M = B * h->cfg.num_objects;
+  const int ntb = int(P.time_blocks.size()), ncb = int(P.ctx_blocks.size()), nxl = int(P.xattn_layers.size());
+  const void* src = nullptr;
+  bool wide = true;      // fp32 source; otherwise the step's activation dtype
+  int r = 0, w = 0;
+  switch (kind) {
+    case DS_TRAIN_ACT:
+    case DS_TRAIN_GRAD:
+      if (index < 0 || index >= int(P.buf_width.size())) return fail(DS_ERR_INVALID, "buffer index %d out of range", index);
+      src = kind == DS_TRAIN_ACT ? t->bufs[index] : t->gbufs[index];
+      wide = !t->bf16;
+      r = M; w = P.buf_width[index];
+      break;
+    case DS_TRAIN_DW:
+      if (index < 0 || index >= int(P.wmats.size())) return fail(DS_ERR_INVALID, "weight matrix index %d out of range", index);
+      src = t->dwarena + t->dw_off[index];
+      r = P.wmats[index].N; w = P.wmats[index].K;
+      break;
+    case DS_TRAIN_DVEC:
+      if (index < 0 || index >= int(P.vecs.size())) return fail(DS_ERR_INVALID, "vector index %d out of range", index);
+      src = t->dvarena + t->v_off[index];
+      r = 1; w = P.vecs[index].n;
+      break;
+    case DS_TRAIN_COND: {
+      const int E = h->cfg.cond_dim, cr = t->last_ctx_rows;
+      switch (index) {
+        case DS_TRAIN_EMB: src = t->emb; r = B; w = C; break;
+        case DS_TRAIN_Z1: src = t->z1; r = B; w = 4 * C; break;
+        case DS_TRAIN_H1: src = t->h1; r = B; w = 4 * C; break;
+        case DS_TRAIN_TEMB: src = t->temb; r = B; w = 4 * C; break;
+        case DS_TRAIN_ST: src = t->st; r = B; w = 4 * C; break;
+        case DS_TRAIN_FILM: src = t->film; r = B; w = ntb * 2 * C; break;
+        case DS_TRAIN_DFILM: src = t->dfilm; r = B; w = ntb * 2 * C; break;
+        case DS_TRAIN_DTEMB: src = t->dtemb; r = B; w = 4 * C; break;
+        case DS_TRAIN_DH1: src = t->dh1; r = B; w = 4 * C; break;
+        case DS_TRAIN_DST: src = t->dst; r = B; w = 4 * C; break;
+        case DS_TRAIN_CTX_ACT: src = t->ctx_act; r = cr; w = E; break;
+        case DS_TRAIN_CTX_FILM: src = t->ctx_film; r = cr; w = ncb * 2 * C; break;
+        case DS_TRAIN_DCTX_FILM: src = t->dctx_film; r = cr; w = ncb * 2 * C; break;
+        case DS_TRAIN_DCTX_ACT: src = t->dctx_act; r = cr; w = E; break;
+        case DS_TRAIN_XKV: src = t->xkv; r = nxl * B * t->last_L; w = 256; break;
+        case DS_TRAIN_XCTX: src = t->xctx; r = nxl * B; w = 4096; break;
+        case DS_TRAIN_XT: src = t->x_t; r = M; w = P.d; break;
+        default: return fail(DS_ERR_INVALID, "conditioning array %d out of range", index);
+      }
+      if (!src || r == 0) return fail(DS_ERR_INVALID, "conditioning array %d is not part of this network's step", index);
+      break;
+    }
+    default:
+      return fail(DS_ERR_INVALID, "bad training-state kind %d", kind);
+  }
+  if (rows) *rows = r;
+  if (width) *width = w;
+  const int64_t n = (int64_t)r * w;
+  if (!dev_out) return 0;      // size query
+  if (n > capacity) return fail(DS_ERR_INVALID, "output capacity %lld < %lld", (long long)capacity, (long long)n);
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (wide) CK(cudaMemcpyAsync(dev_out, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+  else if (n > 0) k_widen_bf16<<<(n + 255) / 256, 256, 0, s>>>((const ds::bf16*)src, dev_out, n);
+  CK(cudaGetLastError());
   return 0;
 }
 

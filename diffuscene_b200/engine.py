@@ -309,6 +309,19 @@ class DenoiserEngine:
         capi.check(self.lib.ds_train_phase_ms(self.h, out))
         return dict(zip(("pack", "forward", "loss", "backward", "cond_paths", "unpack"), [float(v) for v in out]))
 
+    def train_read(self, kind: int, index) -> torch.Tensor:
+        """One array of the training state after the last train_step with gradients (ds_train_read), fp32 on the
+        device: kind is capi.DS_TRAIN_*, index a buffer / weight matrix / vector id of the train plan, or for
+        DS_TRAIN_COND a name of capi.TRAIN_COND."""
+        if kind == capi.DS_TRAIN_COND and isinstance(index, str):
+            index = capi.TRAIN_COND[index]
+        r, w = C.c_int32(), C.c_int32()
+        capi.check(self.lib.ds_train_read(self.h, kind, int(index), None, 0, C.byref(r), C.byref(w), self._stream()))
+        out = torch.empty(r.value * w.value, device=self.device, dtype=torch.float32)
+        capi.check(self.lib.ds_train_read(self.h, kind, int(index), _ptr(out), out.numel(), C.byref(r), C.byref(w),
+                                          self._stream()))
+        return out[: r.value * w.value].view(r.value, w.value)
+
     # ---- debugging ------------------------------------------------------------------------------
     def enable_taps(self, on: bool = True):
         capi.check(self.lib.ds_enable_taps(self.h, int(on)))

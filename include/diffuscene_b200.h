@@ -252,6 +252,32 @@ DS_API int ds_train_set_buckets(ds_handle* h, const int64_t* bounds, int32_t n_b
  * weight packing, forward, loss + d(loss)/d(output), backward through the step program, conditioning paths,
  * gradient unpacking (weight-standardisation adjoint). */
 DS_API int ds_train_phase_ms(ds_handle* h, float* out6);
+/* Arrays of the training state ds_train_read copies (`kind`), and what `index` selects for each:
+ *   DS_TRAIN_ACT   activation buffer `index` of the train step program (ds_plan_export_json with train = 1,
+ *                  no_reuse = 1: every op output has its own buffer), [B*N, width]
+ *   DS_TRAIN_GRAD  the gradient buffer of the same activation after the backward pass, [B*N, width]
+ *   DS_TRAIN_DW    packed gradient of weight matrix `index` (the plan's wmats), [N, K], before the
+ *                  weight-standardisation adjoint
+ *   DS_TRAIN_DVEC  gradient of fp32 vector `index` (the plan's vecs), [1, n]
+ *   DS_TRAIN_COND  one array of the fp32 conditioning paths, `index` from the DS_TRAIN_COND_* list below */
+enum { DS_TRAIN_ACT = 0, DS_TRAIN_GRAD = 1, DS_TRAIN_DW = 2, DS_TRAIN_DVEC = 3, DS_TRAIN_COND = 4 };
+/* [B, C] sinusoidal time embedding; [B, 4C] time_mlp.1 output z1, its GELU h1, time_mlp.3 output temb and SiLU(temb)
+ * st; [B, time blocks x 2C] time-FiLM rows film and their gradient dfilm; [B, 4C] d(temb), d(h1) and dst -- after the
+ * step dst holds d(z1), not d(st); [context rows, cond_dim] SiLU(context) and its gradient; [context rows, context
+ * blocks x 2C] context-FiLM rows and their gradient; text networks: [layers x B x L, 256] text-side kv and
+ * [layers x B, 4096] per-head contexts; [B*N, d] the noisy input x_t the step computed (q_sample, fp32). */
+enum {
+  DS_TRAIN_EMB = 0, DS_TRAIN_Z1, DS_TRAIN_H1, DS_TRAIN_TEMB, DS_TRAIN_ST, DS_TRAIN_FILM, DS_TRAIN_DFILM, DS_TRAIN_DTEMB,
+  DS_TRAIN_DH1, DS_TRAIN_DST, DS_TRAIN_CTX_ACT, DS_TRAIN_CTX_FILM, DS_TRAIN_DCTX_FILM, DS_TRAIN_DCTX_ACT, DS_TRAIN_XKV,
+  DS_TRAIN_XCTX, DS_TRAIN_XT
+};
+/* After a ds_train_step[_cross] with gradients: copy one array of the training state, widened to fp32, into
+ * dev_out [rows, width] on `stream` (profiling / test aid; the step itself is unchanged).  Rows are those of the last
+ * step (B, its context rows, its text length).  DS_ERR_STATE before any step with gradients; DS_ERR_INVALID for a bad
+ * kind or index, an array the network does not have, or capacity < rows * width floats.  dev_out == NULL: a
+ * size query, only rows and width are set. */
+DS_API int ds_train_read(ds_handle* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity,
+                         int32_t* rows, int32_t* width, void* stream);
 /* out[0] += sum(g^2) (device scalar; the caller zeroes it) -- the global gradient norm of clip_grad_norm_. */
 DS_API int ds_sumsq(const float* g_dev, int64_t n, float* out_dev, void* stream);
 /* torch.optim.Adam (weight decay 0, networks/__init__.py:15-34) on flat buffers.  sumsq_dev (optional): device

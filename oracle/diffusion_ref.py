@@ -196,7 +196,7 @@ def iou3d_pairwise(boxes: Tensor, eps: float = 1e-6) -> Tensor:
     ilo = torch.max(lo[:, :, None, :], lo[:, None, :, :])
     ihi = torch.min(hi[:, :, None, :], hi[:, None, :, :])
     inter = (ihi - ilo).clamp(min=0).prod(dim=-1)
-    union = torch.max(vol[:, :, None] + vol[:, None, :] - inter, torch.tensor([eps]))
+    union = torch.max(vol[:, :, None] + vol[:, None, :] - inter, torch.tensor([eps], dtype=vol.dtype, device=vol.device))
     return inter / union
 
 
@@ -215,9 +215,12 @@ class LossSpec:
     room_arrange_condition: bool = False
 
 
-def p_losses(s: Schedule, ls: LossSpec, denoise: DenoiseFn, x0: Tensor, t: Tensor, noise: Tensor):
-    """:520-652, loss_type 'mse'. Returns (losses [B], dict of scalar means)."""
-    x_t = q_sample(s, x0, t, noise)
+def p_losses(s: Schedule, ls: LossSpec, denoise: DenoiseFn, x0: Tensor, t: Tensor, noise: Tensor,
+             x_t: Optional[Tensor] = None):
+    """:520-652, loss_type 'mse'. Returns (losses [B], dict of scalar means).  The schedule tables may live on the
+    device of x0; x_t, when given, replaces q_sample(x0, t, noise) (the noisy input as a caller computed it)."""
+    if x_t is None:
+        x_t = q_sample(s, x0, t, noise)
     target = {"eps": noise, "x0": x0, "v": v_target(s, x0, t, noise)}[s.mean_type]
     out = denoise(x_t, t)
     sq = (target - out) ** 2
@@ -237,7 +240,7 @@ def p_losses(s: Schedule, ls: LossSpec, denoise: DenoiseFn, x0: Tensor, t: Tenso
         l_ob = m(bb + cd - 1, bb + cd)
     else:
         l_ob = m(bb + cd, bb + cd + ls.objectness_dim)
-    l_of = m(bb + cd + ls.objectness_dim, sq.shape[-1]) if ls.objfeat_dim > 0 else torch.zeros(x0.shape[0])
+    l_of = m(bb + cd + ls.objectness_dim, sq.shape[-1]) if ls.objfeat_dim > 0 else x0.new_zeros(x0.shape[0])
     if ls.loss_separate:
         losses = l_bb + l_cl
         if ls.objectness_dim > 0:
@@ -254,8 +257,9 @@ def p_losses(s: Schedule, ls: LossSpec, denoise: DenoiseFn, x0: Tensor, t: Tenso
             valid = (xr[:, :, bb + cd] >= 0).float()
         else:
             valid = (xr[:, :, bb + cd - 1] <= 0).float()
-        tmin, tmax = torch.tensor(ls.bounds_translations[:3]), torch.tensor(ls.bounds_translations[3:])
-        smin, smax = torch.tensor(ls.bounds_sizes[:3]), torch.tensor(ls.bounds_sizes[3:])
+        bt = lambda v: torch.tensor(v, device=x0.device)
+        tmin, tmax = bt(ls.bounds_translations[:3]), bt(ls.bounds_translations[3:])
+        smin, smax = bt(ls.bounds_sizes[:3]), bt(ls.bounds_sizes[3:])
         tr = (xr[:, :, :td] + 1) / 2 * (tmax - tmin) + tmin
         sz = (xr[:, :, td:td + sd_] + 1) / 2 * (smax - smin) + smin
         iou = iou3d_pairwise(torch.cat([tr - sz, tr + sz], dim=-1))
@@ -267,8 +271,8 @@ def p_losses(s: Schedule, ls: LossSpec, denoise: DenoiseFn, x0: Tensor, t: Tenso
         l_iou = (w * 0.1 * iou_valid).sum(dim=(1, 2)) / denom
         losses = losses + l_iou
     else:
-        l_iou = torch.zeros(B)
-        iou_avg = torch.zeros(B)
+        l_iou = x0.new_zeros(B)
+        iou_avg = x0.new_zeros(B)
     return losses, {
         "loss.bbox": l_bb.mean(), "loss.trans": l_tr.mean(), "loss.size": l_sz.mean(),
         "loss.angle": l_an.mean(), "loss.class": l_cl.mean(), "loss.object": l_ob.mean(),

@@ -154,6 +154,15 @@ def eval_op(op: dict, bufs, tb: PlanTables, emulate_bf16: bool = False, inner=No
         out = bufs[op["out"]].clone()
         out[:, op["out_col"]:op["out_col"] + op["N"]] = _r(y, bf)
         return out
+    if k == OP_ACT:      # train program: the activation of a `<name>.pre` GEMM's column slice, other columns kept
+        c0, c1 = op["out_col"], op["out_col"] + op["N"]
+        z = bufs[i0["buf"]][:, i0["col"]:i0["col"] + i0["k"]]
+        y = F.gelu(z) if op["act"] == 1 else F.silu(z)
+        if op["res"] >= 0:
+            y = y + bufs[op["res"]][:, c0:c1]
+        out = bufs[op["out"]].clone()
+        out[:, c0:c1] = _r(y, bf)
+        return out
     if k == OP_GN:
         y = _gn_film_silu(op, bufs[i0["buf"]], tb)
         if op["res"] >= 0:

@@ -30,7 +30,7 @@ def _w2(sd, key):
 def sinusoidal_embedding(t: Tensor, dim: int) -> Tensor:
     """denoise_net.py:127-139: [sin(t*f_k) | cos(t*f_k)], f_k = exp(-k*ln(1e4)/(dim/2-1))."""
     half = dim // 2
-    freq = torch.exp(torch.arange(half, dtype=torch.float32) * -(math.log(10000) / (half - 1)))
+    freq = torch.exp(torch.arange(half, dtype=torch.float32, device=t.device) * -(math.log(10000) / (half - 1)))
     ang = t.to(torch.float32)[:, None] * freq[None, :]
     return torch.cat([ang.sin(), ang.cos()], dim=-1)
 
@@ -167,7 +167,8 @@ def mlp3(sd, name: str, x: Tensor) -> Tensor:
 
 def time_embedding(sd, t: Tensor, dim: int, prefix: str = P) -> Tensor:
     """`time_mlp` (denoise_net.py:417-422): sinusoid -> Linear -> GELU -> Linear."""
-    e = sinusoidal_embedding(t, dim)
+    w1 = sd[prefix + "time_mlp.1.weight"]
+    e = sinusoidal_embedding(t, dim).to(w1.dtype)      # fp32 as in the reference; widened for an fp64 evaluation
     e = F.gelu(F.linear(e, sd[prefix + "time_mlp.1.weight"], sd[prefix + "time_mlp.1.bias"]))
     return F.linear(e, sd[prefix + "time_mlp.3.weight"], sd[prefix + "time_mlp.3.bias"])
 
@@ -182,7 +183,7 @@ def unet1d_forward(sd: Dict[str, Tensor], spec, x: Tensor, t: Tensor, context: O
     """
     sdp = {k[len(prefix):]: v for k, v in sd.items() if k.startswith(prefix)}
     s = spec
-    x = x.to(torch.float32)
+    x = x if x.dtype == torch.float64 else x.to(torch.float32)      # fp64 for a high-precision evaluation
     b0 = s.bbox_dim
     if s.seperate_all:
         c0 = b0 + s.class_dim
