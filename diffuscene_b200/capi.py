@@ -63,6 +63,10 @@ class DsVggConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("precision", "capacity", "device")] + [("reserved", C.c_int32 * 5)]
 
 
+class DsInceptionConfig(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("precision", "capacity", "device")] + [("reserved", C.c_int32 * 5)]
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -163,6 +167,15 @@ def load(rebuild: bool = False):
         "ds_manifold_distances": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p]),
         "ds_manifold_radii": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, p, p]),
         "ds_manifold_cover": (C.c_int, [p, p, C.c_int32, p, p, C.c_int32, C.c_int32, p, p, p, p, p]),
+        "ds_inception_create": (C.c_int, [C.POINTER(DsInceptionConfig), C.POINTER(H)]),
+        "ds_inception_destroy": (C.c_int, [H]),
+        "ds_inception_expected_weight_count": (C.c_int, [H]),
+        "ds_inception_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+        "ds_inception_set_weights": (C.c_int, [H, p, C.c_int64, p]),
+        "ds_inception_features": (C.c_int, [H, p, C.c_int32, C.c_int32, C.c_int32, p, p]),
+        "ds_inception_test_conv": (C.c_int, [C.c_int32, p] + [C.c_int32] * 10 + [p, p, p, C.c_int32, C.c_int32, p]),
+        "ds_feature_stats": (C.c_int, [p, C.c_int32, C.c_int32, p, p, p]),
+        "ds_kid_terms": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, C.c_int32, C.c_int32, p, p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -187,7 +200,10 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_text_enc_expected_weight_count", "ds_text_enc_expected_weight", "ds_text_enc_set_weights",
             "ds_text_enc_forward", "ds_scene_boxes", "ds_scene_stats", "ds_vgg_create", "ds_vgg_destroy",
             "ds_vgg_expected_weight_count", "ds_vgg_expected_weight", "ds_vgg_set_weights", "ds_vgg_features",
-            "ds_vgg_test_conv", "ds_manifold_distances", "ds_manifold_radii", "ds_manifold_cover"]
+            "ds_vgg_test_conv", "ds_manifold_distances", "ds_manifold_radii", "ds_manifold_cover",
+            "ds_inception_create", "ds_inception_destroy", "ds_inception_expected_weight_count",
+            "ds_inception_expected_weight", "ds_inception_set_weights", "ds_inception_features",
+            "ds_inception_test_conv", "ds_feature_stats", "ds_kid_terms"]
 
 
 class DsError(RuntimeError):

@@ -136,4 +136,23 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return fmaf(h, t, h);
 }
 
+// Implicit-GEMM convolution on wgmma (k_vgg_conv, vgg16.cu), stride 1: output pixel (y, x) reads input pixel
+// (y + ky - ph, x + kx - pw) for tap (ky, kx) = (tap / kw, tap % kw).  Output channels [0, cout) land at
+// out[pixel * ldo + co_off + c]; columns of a tile at or past cout are never stored.
+struct VgConvEpi {
+  const float* bias;   // [cout]
+  bf16* out;           // NHWC [B, Ho (/ 2), Wo (/ 2), ldo]
+  int H, W, C, cout;   // input geometry; C is the channel count of one tap's K blocks (a multiple of 64)
+  int taps, kw, ph, pw;
+  int Ho, Wo, ldo, co_off;
+  int tiles_x, tiles_y;
+};
+int conv_tc_set_attrs();
+// tensor maps of the NHWC bf16 input [images, H, W, C] (C % 8 == 0; channels past C read as zero) and of the packed
+// weights [cout, K] (K % 64 == 0); bn is the tile width, 64 or 128
+int conv_tc_maps(CUtensorMap* tm_in, CUtensorMap* tm_w, const void* in, int C, int H, int W, int images,
+                 const bf16* wp, int K, int cout, int bn, char* err, int err_len);
+void conv_tc_launch(const CUtensorMap& tm_in, const CUtensorMap& tm_w, const VgConvEpi& e, int bn, bool pool, int B,
+                    cudaStream_t s);
+
 }  // namespace ds

@@ -75,14 +75,6 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
-struct VgConvEpi {
-  const float* bias;
-  bf16* out;           // NHWC [B, H or H / 2, W or W / 2, cout]
-  int H, W, C, cout;   // input geometry (output is H x W before the pool)
-  int taps;            // 9 (3 x 3, pad 1) or 1 (the first layer's im2col columns)
-  int tiles_x, tiles_y;
-};
-
 template <int BN, bool POOL>
 __global__ void __launch_bounds__(VG_THREADS, 2)
 k_vgg_conv(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CUtensorMap tm_w, VgConvEpi e,
@@ -98,7 +90,7 @@ k_vgg_conv(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CU
   float* const sbias = reinterpret_cast<float*>(base_ptr + S::BIAS_OFF);
 
   const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
-  const int n_tiles = e.cout / BN;
+  const int n_tiles = (e.cout + BN - 1) / BN;
   int t = blockIdx.x;
   const int nt = t % n_tiles; t /= n_tiles;
   const int tx = t % e.tiles_x; t /= e.tiles_x;
@@ -118,12 +110,12 @@ k_vgg_conv(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CU
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  for (int c = tid; c < BN; c += VG_THREADS) sbias[c] = __ldg(e.bias + n0 + c);
+  for (int c = tid; c < BN; c += VG_THREADS) sbias[c] = n0 + c < e.cout ? __ldg(e.bias + n0 + c) : 0.f;
   __syncthreads();
 
   auto issue = [&](int i) {
     const int s = i % VG_STAGES, tap = i / cblocks, cb = i % cblocks;
-    const int dy = e.taps == 9 ? tap / 3 - 1 : 0, dx = e.taps == 9 ? tap % 3 - 1 : 0;
+    const int dy = tap / e.kw - e.ph, dx = tap % e.kw - e.pw;
     const uint32_t sa = base + uint32_t(s * S::STAGE);
     mbar_expect_tx(full_bar(s), S::STAGE);
     tma_load_4d(sa, &tm_in, cb * BK, x0 + dx, y0 + dy, img, full_bar(s));
@@ -195,8 +187,8 @@ k_vgg_conv(const __grid_constant__ CUtensorMap tm_in, const __grid_constant__ CU
   } else {
     for (int idx = tid; idx < BM * CH; idx += VG_THREADS) {
       const int c = (idx % CH) * 8, r = idx / CH, y = y0 + r / VG_TX, x = x0 + r % VG_TX;
-      if (y >= e.H || x >= e.W) continue;
-      *reinterpret_cast<uint4*>(e.out + (((int64_t)img * e.H + y) * e.W + x) * e.cout + n0 + c) =
+      if (y >= e.Ho || x >= e.Wo || n0 + c >= e.cout) continue;
+      *reinterpret_cast<uint4*>(e.out + (((int64_t)img * e.Ho + y) * e.Wo + x) * e.ldo + e.co_off + n0 + c) =
           *reinterpret_cast<const uint4*>(stg + r * S::STG_PITCH + c);
     }
   }
@@ -363,29 +355,13 @@ void conv_geom(VgConv& c, int cin, int cout, int H, int W, bool pool) {
 // packed weights at wp + c.wp_off
 int conv_maps(VgConv& c, const void* in, const bf16* wp, int cap, int l) {
   char err[256] = "";
-  const int C = c.cin == 3 ? 64 : c.cin;
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)c.W, (cuuint64_t)c.H, (cuuint64_t)cap};
-  const cuuint64_t str[3] = {(cuuint64_t)C * 2, (cuuint64_t)c.W * C * 2, (cuuint64_t)c.H * c.W * C * 2};
-  const cuuint32_t box[4] = {BK, VG_TX, VG_TY, 1};
-  if (!encode(&c.tm_in, in, 4, dims, str, box, err, sizeof err))
-    return fail(DS_ERR_CUDA, "vgg16: input tensor map of conv %d: %s", l, err);
-  const cuuint64_t wd[2] = {(cuuint64_t)c.g.Kp, (cuuint64_t)c.cout};
-  const cuuint64_t ws[1] = {(cuuint64_t)c.g.Kp * 2};
-  const cuuint32_t wb[2] = {BK, (cuuint32_t)(c.cout == 64 ? 64 : 128)};
-  if (!encode(&c.tm_w, wp + c.wp_off, 2, wd, ws, wb, err, sizeof err))
-    return fail(DS_ERR_CUDA, "vgg16: weight tensor map of conv %d: %s", l, err);
+  if (conv_tc_maps(&c.tm_in, &c.tm_w, in, c.cin == 3 ? 64 : c.cin, c.H, c.W, cap, wp + c.wp_off, c.g.Kp, c.cout,
+                   c.cout == 64 ? 64 : 128, err, sizeof err))
+    return fail(DS_ERR_CUDA, "vgg16: tensor maps of conv %d: %s", l, err);
   return 0;
 }
 
-int vg_set_attrs() {
-  char err[256] = "";
-  if (!tc_runtime_available(err, sizeof err)) return fail(DS_ERR_CUDA, "%s", err);
-  CK(cudaFuncSetAttribute(k_vgg_conv<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<64>::BYTES));
-  CK(cudaFuncSetAttribute(k_vgg_conv<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<64>::BYTES));
-  CK(cudaFuncSetAttribute(k_vgg_conv<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<128>::BYTES));
-  CK(cudaFuncSetAttribute(k_vgg_conv<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<128>::BYTES));
-  return 0;
-}
+int vg_set_attrs() { return conv_tc_set_attrs(); }
 
 // tensor maps and GEMM plans of the bf16 path over the pass buffers
 int vg_plan_bf16(ds_vgg* h) {
@@ -412,20 +388,15 @@ int vg_plan_bf16(ds_vgg* h) {
   return 0;
 }
 
-template <int BN, bool POOL>
-int launch_conv(const VgConv& c, bf16* out, const float* bias, int B, cudaStream_t s) {
-  VgConvEpi e;
-  e.bias = bias; e.out = out; e.H = c.H; e.W = c.W; e.C = c.g.Kp / (c.cin == 3 ? 1 : 9); e.cout = c.cout;
-  e.taps = c.cin == 3 ? 1 : 9;
-  e.tiles_x = (c.W + VG_TX - 1) / VG_TX;
-  e.tiles_y = (c.H + VG_TY - 1) / VG_TY;
-  const int64_t grid = (int64_t)B * e.tiles_x * e.tiles_y * (c.cout / BN);
-  k_vgg_conv<BN, POOL><<<(unsigned)grid, VG_THREADS, VgSmem<BN>::BYTES, s>>>(c.tm_in, c.tm_w, e, tc_error_flag_dev());
-  return 0;
-}
 void conv_fwd_bf16(const VgConv& c, bf16* out, const float* bias, int B, cudaStream_t s) {
-  if (c.cout == 64) c.pool ? launch_conv<64, true>(c, out, bias, B, s) : launch_conv<64, false>(c, out, bias, B, s);
-  else c.pool ? launch_conv<128, true>(c, out, bias, B, s) : launch_conv<128, false>(c, out, bias, B, s);
+  VgConvEpi e;
+  const bool first = c.cin == 3;
+  e.bias = bias; e.out = out; e.H = c.H; e.W = c.W; e.C = c.g.Kp / (first ? 1 : 9); e.cout = c.cout;
+  e.taps = first ? 1 : 9;
+  e.kw = first ? 1 : 3;
+  e.ph = e.pw = first ? 0 : 1;
+  e.Ho = c.H; e.Wo = c.W; e.ldo = c.cout; e.co_off = 0;
+  conv_tc_launch(c.tm_in, c.tm_w, e, c.cout == 64 ? 64 : 128, c.pool, B, s);
 }
 
 
@@ -485,6 +456,48 @@ int vg_pass_fp32(ds_vgg* h, int B, float* feat, cudaStream_t s) {
 }
 
 }  // namespace
+
+namespace ds {
+int conv_tc_set_attrs() {
+  char err[256] = "";
+  if (!tc_runtime_available(err, sizeof err)) return fail(DS_ERR_CUDA, "%s", err);
+  CK(cudaFuncSetAttribute(k_vgg_conv<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<64>::BYTES));
+  CK(cudaFuncSetAttribute(k_vgg_conv<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<64>::BYTES));
+  CK(cudaFuncSetAttribute(k_vgg_conv<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<128>::BYTES));
+  CK(cudaFuncSetAttribute(k_vgg_conv<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, VgSmem<128>::BYTES));
+  return 0;
+}
+
+int conv_tc_maps(CUtensorMap* tm_in, CUtensorMap* tm_w, const void* in, int C, int H, int W, int images,
+                 const bf16* wp, int K, int cout, int bn, char* err, int err_len) {
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)images};
+  const cuuint64_t str[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {BK, VG_TX, VG_TY, 1};
+  if (!encode(tm_in, in, 4, dims, str, box, err, err_len)) return -1;
+  const cuuint64_t wd[2] = {(cuuint64_t)K, (cuuint64_t)cout};
+  const cuuint64_t ws[1] = {(cuuint64_t)K * 2};
+  const cuuint32_t wb[2] = {BK, (cuuint32_t)bn};
+  if (!encode(tm_w, wp, 2, wd, ws, wb, err, err_len)) return -1;
+  return 0;
+}
+
+void conv_tc_launch(const CUtensorMap& tm_in, const CUtensorMap& tm_w, const VgConvEpi& e0, int bn, bool pool, int B,
+                    cudaStream_t s) {
+  VgConvEpi e = e0;
+  e.tiles_x = (e.Wo + VG_TX - 1) / VG_TX;
+  e.tiles_y = (e.Ho + VG_TY - 1) / VG_TY;
+  const int64_t grid = (int64_t)B * e.tiles_x * e.tiles_y * ((e.cout + bn - 1) / bn);
+  int* flag = tc_error_flag_dev();
+  if (bn == 64) {
+    if (pool) k_vgg_conv<64, true><<<(unsigned)grid, VG_THREADS, VgSmem<64>::BYTES, s>>>(tm_in, tm_w, e, flag);
+    else k_vgg_conv<64, false><<<(unsigned)grid, VG_THREADS, VgSmem<64>::BYTES, s>>>(tm_in, tm_w, e, flag);
+  } else {
+    if (pool) k_vgg_conv<128, true><<<(unsigned)grid, VG_THREADS, VgSmem<128>::BYTES, s>>>(tm_in, tm_w, e, flag);
+    else k_vgg_conv<128, false><<<(unsigned)grid, VG_THREADS, VgSmem<128>::BYTES, s>>>(tm_in, tm_w, e, flag);
+  }
+}
+
+}  // namespace ds
 
 extern "C" int ds_vgg_create(const ds_vgg_config* cfg, ds_vgg** out) {
   if (!cfg || !out) return fail(DS_ERR_INVALID, "null argument");

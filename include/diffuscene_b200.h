@@ -488,6 +488,61 @@ DS_API int ds_vgg_set_weights(ds_vgg* h, const float* flat_params_dev, int64_t c
 DS_API int ds_vgg_features(ds_vgg* h, const float* images_dev, int32_t batch, int32_t height, int32_t width,
                            float* features_dev, void* stream);
 
+/* ---- FID and KID of rendered scenes ------------------------------------------------------------
+ * Feature extractor: the FID Inception-v3 (clean-fid's `clean` mode as pytorch-fid restates its blocks), the 2048-d
+ * pool3 output of torchvision's Inception3 layout with aux_logits off, where the branch_pool average pools of
+ * Mixed_5b-d, 6b-e and 7b exclude the padding and Mixed_7c's branch_pool is a 3 x 3 / stride 1 / pad 1 max pool.
+ * Every BasicConv2d's BatchNorm (eps 1e-3, running statistics) is folded into its weights when they are set.  fp32
+ * mode runs im2col and the exact SIMT GEMM; bf16 mode runs the convolutions as implicit GEMMs on wgmma (the stride-2
+ * ones and the first over an im2col).  Features are fp32 in both modes.
+ * Parameters are ONE flat fp32 device buffer in ds_inception_expected_weight() order: torchvision
+ * Inception3(aux_logits=False) state-dict names and sizes in state-dict order, without fc.* and
+ * num_batches_tracked (94 x {conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var}). */
+typedef struct ds_inception ds_inception;
+typedef struct ds_inception_config {
+  int32_t precision;        /* ds_precision: fp32 parity mode or bf16 tensor-core mode                          */
+  int32_t capacity;         /* images one internal pass holds, 1 .. 256; larger batches run in passes of this size */
+  int32_t device;           /* CUDA device ordinal                                                               */
+  int32_t reserved[5];
+} ds_inception_config;
+#define DS_INCEPTION_FEATURES 2048
+DS_API int ds_inception_create(const ds_inception_config* cfg, ds_inception** out);
+DS_API int ds_inception_destroy(ds_inception* h);
+DS_API int ds_inception_expected_weight_count(ds_inception* h);
+DS_API int ds_inception_expected_weight(ds_inception* h, int index, const char** name, int64_t* numel);
+/* DS_ERR_INVALID for NULL pointers or a parameter count other than the sum of the expected sizes. */
+DS_API int ds_inception_set_weights(ds_inception* h, const float* flat_params_dev, int64_t count, void* stream);
+/* images [batch, 3, 299, 299] fp32 NCHW in [0, 255] (already resized) -> features [batch, 2048] fp32, device
+ * pointers; the detector's input is (x - 128) / 128.  An image's features do not depend on the other images of the
+ * batch.  DS_ERR_STATE before ds_inception_set_weights; DS_ERR_INVALID for NULL pointers, batch < 0 or a size other
+ * than 299 x 299. */
+DS_API int ds_inception_features(ds_inception* h, const float* images_dev, int32_t batch, int32_t height, int32_t width,
+                                 float* features_dev, void* stream);
+/* One convolution alone, for unit tests, through the kernels, tensor maps and packing ds_inception_features runs in
+ * `precision`: x [batch, height, width, cin] fp32 NHWC (rounded to bf16 in bf16 mode) -> relu(conv(x, W, b)) with
+ * kernel kh x kw, stride 1 or 2 and padding (pad_h, pad_w), W [cout, cin, kh, kw] and b [cout] fp32, written to
+ * channels [out_offset, out_offset + cout) of out [batch, Ho, Wo, out_pitch] fp32; the other channels keep their values
+ * (rounded to bf16 in bf16 mode).  cout, out_pitch and out_offset are multiples of 8.  Synchronises `stream`. */
+DS_API int ds_inception_test_conv(int32_t precision, const float* in_dev, int32_t batch, int32_t height, int32_t width,
+                                  int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride, int32_t pad_h,
+                                  int32_t pad_w, const float* weight_dev, const float* bias_dev, float* out_dev,
+                                  int32_t out_pitch, int32_t out_offset, void* stream);
+
+/* FID statistics of fp32 features [n, d]: mean [d] and cov [d, d] = (X - mean)^T (X - mean) / (n - 1), fp64, as
+ * np.mean / np.cov on float64-promoted features, in a fixed summation order.  DS_ERR_INVALID for NULL pointers,
+ * n < 2 or d < 1.  Stateless. */
+DS_API int ds_feature_stats(const float* feats_dev, int32_t n, int32_t d, double* mean_dev, double* cov_dev,
+                            void* stream);
+/* KID terms of `subsets` subsets of m rows (clean-fid's kernel_distance): for subset s, x = fake[idx_fake[s * m ..]],
+ * y = real[idx_real[s * m ..]] (int64 indices), a = (x x^T / d + 1)^3 + (y y^T / d + 1)^3, b = (x y^T / d + 1)^3 and
+ * terms[s] = (sum a - sum diag a) / (m - 1) - 2 sum b / m, fp64 (KID = sum of terms / subsets / m).  Each term is
+ * deterministic and independent of the other subsets of the call.  The indices are checked on the device first (the
+ * call synchronises `stream` for that); DS_ERR_INVALID for one outside its set, NULL pointers, m < 2, m above either
+ * set's size, subsets < 1 or d < 1.  Scratch is allocated on `stream`. */
+DS_API int ds_kid_terms(const float* real_dev, int32_t n_real, const float* fake_dev, int32_t n_fake, int32_t d,
+                        const int64_t* idx_fake_dev, const int64_t* idx_real_dev, int32_t subsets, int32_t m,
+                        double* terms_dev, void* stream);
+
 /* Manifold metrics (improved_precision_recall.py:196-256) on fp64 features [rows, d] (row-major, any d >= 1), without
  * an N x N matrix: distances are sqrt(max(0, (|x|^2 - 2 x.y) + |y|^2)) in fp64 on the fp64 tensor cores, and
  * `clamped_dev` (int64 on the device, may be NULL) receives how many squared distances were negative and set to 0,

@@ -9,7 +9,6 @@ Without SPLITS_CSV the real set is every *.jpg / *.png under REAL_DIR; with it, 
 random.Random(100) and cut to --num_samples, as the reference does with its temporary copies (none are made here).
 """
 import argparse
-import csv
 import os
 import sys
 
@@ -17,21 +16,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from diffuscene_b200 import ipr as I  # noqa: E402
-
-RENDER_NAMES = ("rendered_scene_256.png", "rendered_scene_256_no_lamps.png", "rendered_scene_notexture_256.png")
-
-
-def real_renders(base_dir, splits_csv):
-    """CachedThreedFront's renders of the train + val scenes: directories `<x>_<scene id>` sorted, one file name
-    chosen from the first directory."""
-    with open(splits_csv) as f:
-        ids = {r[0] for r in csv.reader(f) if len(r) > 1 and r[1] in ("train", "val")}
-    tags = sorted(d for d in os.listdir(base_dir) if len(d.split("_")) > 1 and d.split("_")[1] in ids)
-    if not tags:
-        raise SystemExit("no scene of %s in %s" % (splits_csv, base_dir))
-    name = next((n for n in RENDER_NAMES[:2] if os.path.isfile(os.path.join(base_dir, tags[0], n))), RENDER_NAMES[2])
-    print("rendered_scene is :", name)
-    return sorted(os.path.join(base_dir, t, name) for t in tags)
+from diffuscene_b200.renders import real_renders  # noqa: E402
 
 
 def toy():
