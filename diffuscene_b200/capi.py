@@ -20,6 +20,8 @@ DS_TRAIN_ACT, DS_TRAIN_GRAD, DS_TRAIN_DW, DS_TRAIN_DVEC, DS_TRAIN_COND = range(5
 TRAIN_COND = {n: i for i, n in enumerate((
     "emb", "z1", "h1", "temb", "st", "film", "dfilm", "dtemb", "dh1", "dst", "ctx_act", "ctx_film", "dctx_film",
     "dctx_act", "xkv", "xctx", "x_t"))}      # DS_TRAIN_COND indices (include/diffuscene_b200.h)
+ROOM_ENC_STATE = {n: i for i, n in enumerate((
+    "x0", "a1", "p", "h", "o", "wp", "bias", "dwp", "dbias", "dz", "dh", "dp", "da1"))}      # DS_RE_* kinds
 
 
 class DsConfig(C.Structure):
@@ -140,6 +142,7 @@ def load(rebuild: bool = False):
         "ds_room_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
         "ds_room_enc_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, p]),
         "ds_room_enc_backward": (C.c_int, [H, p, p, p]),
+        "ds_room_enc_read": (C.c_int, [H, C.c_int32, C.c_int32, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), p]),
         "ds_shape_ae_create": (C.c_int, [C.POINTER(DsShapeAeConfig), C.POINTER(H)]),
         "ds_shape_ae_destroy": (C.c_int, [H]),
         "ds_shape_ae_expected_weight_count": (C.c_int, [H]),
@@ -193,7 +196,7 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_train_read", "ds_sumsq", "ds_adam_step",
             "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
             "ds_test_gemm_bf16", "ds_room_enc_create", "ds_room_enc_destroy", "ds_room_enc_expected_weight_count",
-            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_shape_ae_create",
+            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_room_enc_read", "ds_shape_ae_create",
             "ds_shape_ae_destroy", "ds_shape_ae_expected_weight_count", "ds_shape_ae_expected_weight",
             "ds_shape_ae_forward", "ds_shape_ae_train_step", "ds_shape_ae_set_knn", "ds_shape_ae_get_knn", "ds_knn",
             "ds_chamfer_forward", "ds_chamfer_backward", "ds_text_enc_create", "ds_text_enc_destroy",

@@ -101,14 +101,14 @@ void launch_re_col2im(const T* dcols, const RoomConvGeom& g, int B, T* out, int 
   if (n > 0) k_re_col2im<T><<<re_blocks(n, 256), 256, 0, s>>>(dcols, g, out, accumulate, add, mask, n);
 }
 
-// out = relu(z (+ res)); in place allowed (out == z)
+// out = relu(z (+ res)); in place allowed (out == z).  NaN passes through, as torch's relu lets it.
 template <typename T>
 __global__ void k_re_add_relu(const T* z, const T* __restrict__ res, T* out, int64_t n) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   float v = ldf(z + i);
   if (res) v += ldf(res + i);
-  stf(out + i, v > 0.f ? v : 0.f);
+  stf(out + i, (v > 0.f || v != v) ? v : 0.f);
 }
 template <typename T>
 void launch_re_add_relu(const T* z, const T* res, T* out, int64_t n, cudaStream_t s) {
@@ -116,7 +116,8 @@ void launch_re_add_relu(const T* z, const T* res, T* out, int64_t n, cudaStream_
 }
 
 // 3x3 / stride 2 / pad 1 max pool window of output (oy, ox): torch's argmax, i.e. the first maximum in row-major
-// window order (strict >), the padding acting as -inf.  Returns the flat input pixel index within the scene.
+// window order (strict >), the padding acting as -inf.  A NaN is taken as a new maximum, as torch's max_pool2d takes
+// it, so a window holding NaN pools to NaN.  Returns the flat input pixel index within the scene.
 template <typename T>
 __device__ __forceinline__ int re_pool_argmax(const T* in, int64_t b, int oy, int ox, int C, int c, int hin, int win,
                                               float* best_out) {
@@ -129,7 +130,7 @@ __device__ __forceinline__ int re_pool_argmax(const T* in, int64_t b, int oy, in
       const int ix = ox * 2 - 1 + kx;
       if (ix < 0 || ix >= win) continue;
       const float v = ldf(in + ((b * hin + iy) * win + ix) * C + c);
-      if (v > best || arg < 0) {
+      if (v > best || isnan(v) || arg < 0) {
         best = v;
         arg = iy * win + ix;
       }
@@ -318,11 +319,16 @@ struct ds_room_enc {
   // device buffers
   int cap = 0;
   void *x0 = nullptr, *a1 = nullptr, *p = nullptr, *h[8] = {nullptr}, *o[8] = {nullptr};
-  void *cols = nullptr, *z = nullptr, *dsb = nullptr, *gA = nullptr, *gB = nullptr, *gC = nullptr;
+  void *cols = nullptr, *z = nullptr, *dsb = nullptr;
+  // input gradients of the backward pass, one buffer per array (ds_room_enc_read): per block the gradient of the
+  // pre-ReLU block sum (dz) and of conv1's pre-ReLU output (dh); the max-pool output (dp) and input (da1)
+  void *dz[8] = {nullptr}, *dh[8] = {nullptr}, *dp = nullptr, *da1 = nullptr;
   void* wp = nullptr;
   float *bias = nullptr, *dwp = nullptr, *dbias = nullptr;
   size_t wp_total = 0, b_total = 0, dw_total = 0;
   std::vector<TcGemmPlan*> tc;      // forward GEMM plans (bf16, output width % 128 == 0), per conv
+  int last_B = 0;                   // batch of the last forward (0: none since the buffers were allocated)
+  bool have_grads = false;          // a backward ran after the last forward
   // state kept by a forward with keep_for_backward
   bool kept = false;
   int kept_B = 0;
@@ -336,10 +342,13 @@ constexpr int RE_ROW_CHUNK = 32768 * 64;
 void re_free(ds_room_enc* h) {
   for (auto* p : h->tc) if (p) tc_plan_destroy(p);
   h->tc.assign(h->conv.size(), nullptr);
-  void** bufs[] = {&h->x0, &h->a1, &h->p, &h->cols, &h->z, &h->dsb, &h->gA, &h->gB, &h->gC};
+  void** bufs[] = {&h->x0, &h->a1, &h->p, &h->cols, &h->z, &h->dsb, &h->dp, &h->da1};
   for (void** b : bufs) { cudaFree(*b); *b = nullptr; }
-  for (int i = 0; i < 8; ++i) { cudaFree(h->h[i]); cudaFree(h->o[i]); h->h[i] = h->o[i] = nullptr; }
+  for (int i = 0; i < 8; ++i)
+    for (void** b : {&h->h[i], &h->o[i], &h->dz[i], &h->dh[i]}) { cudaFree(*b); *b = nullptr; }
   h->cap = 0;
+  h->last_B = 0;
+  h->have_grads = false;
   h->kept = false;
 }
 
@@ -389,13 +398,13 @@ int re_ensure(ds_room_enc* h, int B) {
   CK(cudaMalloc(&h->p, (size_t)B * h->H4 * h->W4 * 64 * e));
   for (int i = 0; i < 8; ++i) {
     const RoomConvGeom& g = h->conv[h->blk_first[i]].g;
-    CK(cudaMalloc(&h->h[i], (size_t)rows_of(g, B) * g.cout * e));
-    CK(cudaMalloc(&h->o[i], (size_t)rows_of(g, B) * g.cout * e));
+    for (void** b : {&h->h[i], &h->o[i], &h->dz[i], &h->dh[i]}) CK(cudaMalloc(b, (size_t)rows_of(g, B) * g.cout * e));
   }
   CK(cudaMalloc(&h->cols, (size_t)cols_max * e));
   CK(cudaMalloc(&h->z, (size_t)z_max * e));
   CK(cudaMalloc(&h->dsb, (size_t)z_max * e));
-  for (void** g : {&h->gA, &h->gB, &h->gC}) CK(cudaMalloc(g, (size_t)std::max(a1n, z_max) * e));
+  CK(cudaMalloc(&h->dp, (size_t)B * h->H4 * h->W4 * 64 * e));
+  CK(cudaMalloc(&h->da1, (size_t)a1n * e));
   h->cap = B;
   if (h->bf16) {
     char err[256] = "";
@@ -499,17 +508,17 @@ int re_backward(ds_room_enc* h, const float* dfeat, float* grads, cudaStream_t s
   CK(cudaMemsetAsync(grads, 0, (size_t)h->n_params * 4, s));
   CK(cudaMemsetAsync(h->dwp, 0, h->dw_total * 4, s));
   CK(cudaMemsetAsync(h->dbias, 0, h->b_total * 4, s));
-  T* dz = P<T>(h->gA);
-  T* dh = P<T>(h->gB);
-  T* dx = P<T>(h->gC);
   {
     const RoomConvGeom& gl = h->conv[h->blk_first[7] + 1].g;
-    launch_re_avgpool_bwd<T>(dfeat, P<T>(h->o[7]), dz, B, 512, gl.hout * gl.wout, s);
+    launch_re_avgpool_bwd<T>(dfeat, P<T>(h->o[7]), P<T>(h->dz[7]), B, 512, gl.hout * gl.wout, s);
   }
   for (int b = 7; b >= 0; --b) {
     const int f = h->blk_first[b];
     const T* x = b > 0 ? P<T>(h->o[b - 1]) : P<T>(h->p);
     const T* xmask = b > 0 ? x : nullptr;      // the max-pool output gets its ReLU adjoint after the pool adjoint
+    T* dz = P<T>(h->dz[b]);
+    T* dh = P<T>(h->dh[b]);
+    T* dx = b > 0 ? P<T>(h->dz[b - 1]) : P<T>(h->dp);
     conv_bwd_w<T>(h, f + 1, P<T>(h->h[b]), dz, B, true, s);
     launch_re_col2im<T>(P<T>(h->cols), h->conv[f + 1].g, B, dh, 0, nullptr, P<T>(h->h[b]), s);
     conv_bwd_w<T>(h, f, x, dh, B, true, s);
@@ -520,10 +529,9 @@ int re_backward(ds_room_enc* h, const float* dfeat, float* grads, cudaStream_t s
     } else {
       launch_re_col2im<T>(P<T>(h->cols), h->conv[f].g, B, dx, 0, dz, xmask, s);
     }
-    std::swap(dz, dx);
   }
-  launch_re_maxpool_bwd<T>(P<T>(h->a1), dz, dh, B, 64, h->H2, h->W2, h->H4, h->W4, s);
-  conv_bwd_w<T>(h, 0, P<T>(h->x0), dh, B, false, s);
+  launch_re_maxpool_bwd<T>(P<T>(h->a1), P<T>(h->dp), P<T>(h->da1), B, 64, h->H2, h->W2, h->H4, h->W4, s);
+  conv_bwd_w<T>(h, 0, P<T>(h->x0), P<T>(h->da1), B, false, s);
   for (const RConv& c : h->conv)
     launch_re_fold_bwd(h->dwp + c.dw_off, h->dbias + c.b_off, prm + h->off[c.w_idx], prm + h->off[c.bn_idx], c.g,
                        grads + h->off[c.w_idx], grads + h->off[c.bn_idx], s);
@@ -627,6 +635,8 @@ extern "C" int ds_room_enc_forward(ds_room_enc* h, const float* flat_params_dev,
                : re_forward<float>(h, flat_params_dev, mask_dev, batch, feat_dev, s);
   if (rc) return rc;
   CK(cudaGetLastError());
+  h->last_B = batch;
+  h->have_grads = false;
   if (keep_for_backward) {
     h->kept = true;
     h->kept_B = batch;
@@ -643,6 +653,68 @@ extern "C" int ds_room_enc_backward(ds_room_enc* h, const float* dfeat_dev, floa
   const int rc = h->bf16 ? re_backward<bf16>(h, dfeat_dev, flat_grads_dev, s)
                          : re_backward<float>(h, dfeat_dev, flat_grads_dev, s);
   if (rc) return rc;
+  CK(cudaGetLastError());
+  h->have_grads = true;
+  return 0;
+}
+
+namespace {
+__global__ void k_re_widen_bf16(const ds::bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = __bfloat162float(in[i]);
+}
+}  // namespace
+
+extern "C" int ds_room_enc_read(ds_room_enc* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity,
+                                int32_t* rows, int32_t* width, void* stream) {
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  if (!h->last_B) return fail(DS_ERR_STATE, "room encoder: no forward has run");
+  const bool grad_kind = kind >= DS_RE_DWP && kind <= DS_RE_DA1;
+  if (grad_kind && !h->have_grads) return fail(DS_ERR_STATE, "room encoder: no backward since the last forward");
+  const int B = h->last_B;      // a backward always follows the forward it differentiates
+  const int n_conv = int(h->conv.size());
+  const void* src = nullptr;
+  bool wide = false;      // fp32 source; otherwise the handle's activation dtype
+  int64_t r = 0;
+  int w = 0;
+  switch (kind) {
+    case DS_RE_X0:
+      src = h->x0; r = (int64_t)B * h->cfg.height * h->cfg.width; w = h->cfg.input_channels; break;
+    case DS_RE_A1: case DS_RE_DA1:
+      src = kind == DS_RE_A1 ? h->a1 : h->da1; r = (int64_t)B * h->H2 * h->W2; w = 64; break;
+    case DS_RE_P: case DS_RE_DP:
+      src = kind == DS_RE_P ? h->p : h->dp; r = (int64_t)B * h->H4 * h->W4; w = 64; break;
+    case DS_RE_H: case DS_RE_O: case DS_RE_DZ: case DS_RE_DH: {
+      if (index < 0 || index >= 8) return fail(DS_ERR_INVALID, "room encoder: block index %d out of range", index);
+      const RoomConvGeom& g = h->conv[h->blk_first[index]].g;
+      src = kind == DS_RE_H ? h->h[index] : kind == DS_RE_O ? h->o[index] : kind == DS_RE_DZ ? h->dz[index] : h->dh[index];
+      r = rows_of(g, B); w = g.cout;
+      break;
+    }
+    case DS_RE_WP: case DS_RE_BIAS: case DS_RE_DWP: case DS_RE_DBIAS: {
+      if (index < 0 || index >= n_conv) return fail(DS_ERR_INVALID, "room encoder: conv index %d out of range", index);
+      const RConv& c = h->conv[index];
+      const bool vec = kind == DS_RE_BIAS || kind == DS_RE_DBIAS;
+      src = kind == DS_RE_WP ? P<char>(h->wp, c.wp_off * h->esz) : kind == DS_RE_BIAS ? (void*)(h->bias + c.b_off)
+            : kind == DS_RE_DWP ? (void*)(h->dwp + c.dw_off) : (void*)(h->dbias + c.b_off);
+      wide = kind != DS_RE_WP;
+      r = vec ? 1 : c.g.cout; w = vec ? c.g.cout : c.g.Kp;
+      break;
+    }
+    default:
+      return fail(DS_ERR_INVALID, "room encoder: bad state kind %d", kind);
+  }
+  if (!h->bf16) wide = true;
+  if (r > INT32_MAX) return fail(DS_ERR_INVALID, "room encoder: %lld rows do not fit the row count", (long long)r);
+  if (rows) *rows = int32_t(r);
+  if (width) *width = w;
+  const int64_t n = r * w;
+  if (!dev_out) return 0;      // size query
+  if (n > capacity) return fail(DS_ERR_INVALID, "output capacity %lld < %lld", (long long)capacity, (long long)n);
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (wide) CK(cudaMemcpyAsync(dev_out, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+  else if (n > 0) k_re_widen_bf16<<<ds::re_blocks(n, 256), 256, 0, s>>>((const ds::bf16*)src, dev_out, n);
   CK(cudaGetLastError());
   return 0;
 }

@@ -93,6 +93,18 @@ class RoomMaskEncoder:
         capi.check(self.lib.ds_room_enc_backward(self.h, C.c_void_p(dfeat.data_ptr()), C.c_void_p(grads.data_ptr()),
                                                  self._stream()))
 
+    def read(self, kind, index: int = 0) -> torch.Tensor:
+        """One array of the encoder's state (ds_room_enc_read), fp32 [rows, width] on the device: kind is a name of
+        capi.ROOM_ENC_STATE (or its DS_RE_* value), index a block (0 .. 7) or a conv in expected-weight order."""
+        if isinstance(kind, str):
+            kind = capi.ROOM_ENC_STATE[kind]
+        r, w = C.c_int32(), C.c_int32()
+        capi.check(self.lib.ds_room_enc_read(self.h, kind, int(index), None, 0, C.byref(r), C.byref(w), self._stream()))
+        out = torch.empty(r.value, w.value, device=self.device, dtype=torch.float32)
+        capi.check(self.lib.ds_room_enc_read(self.h, kind, int(index), C.c_void_p(out.data_ptr()), out.numel(),
+                                             C.byref(r), C.byref(w), self._stream()))
+        return out
+
     def close(self):
         if self.h:
             self.lib.ds_room_enc_destroy(self.h)

@@ -367,6 +367,35 @@ DS_API int ds_room_enc_forward(ds_room_enc* h, const float* flat_params_dev, con
 /* d(loss)/d(feat) [batch, 512] of the kept forward -> flat_grads_dev (same layout as the parameters, overwritten;
  * the running statistics get 0).  DS_ERR_INVALID when no forward was kept. */
 DS_API int ds_room_enc_backward(ds_room_enc* h, const float* dfeat_dev, float* flat_grads_dev, void* stream);
+/* Arrays of the encoder's state ds_room_enc_read copies (`kind`), and what `index` selects.  Rows are those of the
+ * last forward (B scenes; an H x W mask, H2 = H / 2, H4 = H / 4); activations are NHWC rows (scene, y, x) x channels.
+ * Convs are numbered in ds_room_enc_expected_weight order: 0 the stem, then per block conv1, conv2 (, downsample).
+ *   after a forward:
+ *   DS_RE_X0     the packed mask, [B H W, input_channels]
+ *   DS_RE_A1     the stem output after its ReLU, [B H2 W2, 64]
+ *   DS_RE_P      the max-pool output, [B H4 W4, 64]
+ *   DS_RE_H      block `index` (0 .. 7): conv1's output after its ReLU, [block rows, block width]
+ *   DS_RE_O      block `index`: the block output relu(conv2 + residual)
+ *   DS_RE_WP     conv `index`: the folded weight W' the kernels read, [cout, Kp] (columns (ky, kx, cin), zero past
+ *                k k cin up to Kp, a multiple of 64)
+ *   DS_RE_BIAS   conv `index`: the folded fp32 bias, [1, cout]
+ *   after a backward (and no forward since):
+ *   DS_RE_DWP    conv `index`: dW' [cout, Kp], before the adjoint of the fold
+ *   DS_RE_DBIAS  conv `index`: d(bias) [1, cout]
+ *   DS_RE_DZ     block `index`: the gradient of the block's pre-ReLU sum conv2 + residual
+ *   DS_RE_DH     block `index`: the gradient of conv1's pre-ReLU output
+ *   DS_RE_DP     the gradient of the max-pool output
+ *   DS_RE_DA1    the gradient of the stem's pre-ReLU output (the max-pool adjoint, masked by the stem's ReLU) */
+enum {
+  DS_RE_X0 = 0, DS_RE_A1, DS_RE_P, DS_RE_H, DS_RE_O, DS_RE_WP, DS_RE_BIAS, DS_RE_DWP, DS_RE_DBIAS, DS_RE_DZ, DS_RE_DH,
+  DS_RE_DP, DS_RE_DA1
+};
+/* Copy one array of the encoder's state, widened to fp32, into dev_out [rows, width] on `stream` (test / profiling
+ * aid; forward and backward are unchanged by it).  DS_ERR_STATE before any forward, and for the gradient kinds when no
+ * backward ran after the last forward; DS_ERR_INVALID for a bad kind or index, or capacity < rows * width floats.
+ * dev_out == NULL: a size query, only rows and width are set. */
+DS_API int ds_room_enc_read(ds_room_enc* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity,
+                            int32_t* rows, int32_t* width, void* stream);
 
 /* ---- object shape auto-encoder ---------------------------------------------------------------
  * The reference's KLAutoEncoder (scene_synthesis/networks/foldingnet_autoencoder.py:131-390): a FoldingNet encoder
