@@ -16,8 +16,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdiffuscene_b200.so")
-SOURCES = ["engine.cu", "plan.cpp", "pointwise.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_ln.cu", "gemm_attn.cu", "backward.cu", "train.cu", "room_encoder.cu", "shape_ae.cu", "text_encoder.cu", "scene_eval.cu", "vgg16.cu", "manifold.cu", "inception.cu", "fid_stats.cu"]
-HEADERS = ["common.cuh", "kernels.cuh", "tc_common.cuh", "plan.h", "engine_internal.h", os.path.join("..", "..", "include", "diffuscene_b200.h")]
+SOURCES = ["engine.cu", "plan.cpp", "pointwise.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_ln.cu", "gemm_attn.cu", "backward.cu", "train.cu", "room_encoder.cu", "shape_ae.cu", "text_encoder.cu", "scene_eval.cu", "vgg16.cu", "manifold.cu", "inception.cu", "fid_stats.cu", "render.cu", "resize.cu"]
+HEADERS = ["common.cuh", "kernels.cuh", "tc_common.cuh", "placement.cuh", "plan.h", "engine_internal.h", os.path.join("..", "..", "include", "diffuscene_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

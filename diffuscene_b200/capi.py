@@ -69,6 +69,25 @@ class DsInceptionConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("precision", "capacity", "device")] + [("reserved", C.c_int32 * 5)]
 
 
+class DsRenderCamera(C.Structure):
+    _fields_ = [("eye", C.c_float * 3), ("target", C.c_float * 3), ("up", C.c_float * 3)] + \
+        [(n, C.c_float) for n in ("left", "right", "bottom", "top", "near_plane", "far_plane")] + \
+        [("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32 * 4)]
+
+
+class DsRenderArgs(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_objects", C.c_int32)] + \
+        [(n, C.c_void_p) for n in ("translation_dev", "size_dev", "angle_dev", "model_index_dev", "class_index_dev",
+                                   "floor_offsets_dev", "floor_tris_dev")] + \
+        [("num_floor_tris", C.c_int32), ("num_colors", C.c_int32), ("palette_dev", C.c_void_p),
+         ("floor_textures_dev", C.c_void_p), ("num_floor_textures", C.c_int32), ("floor_texture_size", C.c_int32),
+         ("floor_texture_index_dev", C.c_void_p), ("flags", C.c_int32), ("reserved0", C.c_int32),
+         ("image_dev", C.c_void_p), ("id_dev", C.c_void_p), ("reserved", C.c_int32 * 8)]
+
+
+DS_RENDER_NO_TEXTURE, DS_RENDER_WHITE_BACKGROUND = 1, 2
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -179,6 +198,11 @@ def load(rebuild: bool = False):
         "ds_inception_test_conv": (C.c_int, [C.c_int32, p] + [C.c_int32] * 10 + [p, p, p, C.c_int32, C.c_int32, p]),
         "ds_feature_stats": (C.c_int, [p, C.c_int32, C.c_int32, p, p, p]),
         "ds_kid_terms": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, C.c_int32, C.c_int32, p, p]),
+        "ds_mesh_catalog_create": (C.c_int, [C.c_int32, p, p, p, p, p, p, p, p, p, C.c_int32, C.c_int32, C.POINTER(H)]),
+        "ds_mesh_catalog_destroy": (C.c_int, [H]),
+        "ds_render_scenes": (C.c_int, [H, C.POINTER(DsRenderCamera), C.POINTER(DsRenderArgs), p]),
+        "ds_resize_f32": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p]),
+        "ds_resize_u8": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p, p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -206,7 +230,8 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_vgg_test_conv", "ds_manifold_distances", "ds_manifold_radii", "ds_manifold_cover",
             "ds_inception_create", "ds_inception_destroy", "ds_inception_expected_weight_count",
             "ds_inception_expected_weight", "ds_inception_set_weights", "ds_inception_features",
-            "ds_inception_test_conv", "ds_feature_stats", "ds_kid_terms"]
+            "ds_inception_test_conv", "ds_feature_stats", "ds_kid_terms", "ds_mesh_catalog_create",
+            "ds_mesh_catalog_destroy", "ds_render_scenes", "ds_resize_f32", "ds_resize_u8"]
 
 
 class DsError(RuntimeError):

@@ -5,6 +5,7 @@
 // Every operation is an explicit _rn intrinsic, so no FMA contraction changes a result, and every sum runs in a fixed
 // order without atomics: a scene's numbers do not depend on the batch it is evaluated in.
 #include "engine_internal.h"
+#include "placement.cuh"
 
 namespace ds {
 namespace {
@@ -17,11 +18,11 @@ enum { SE_ERR_OFFSETS = 1, SE_ERR_INDEX = 2 };
 
 inline int cdiv(int64_t a, int64_t b) { return int((a + b - 1) / b); }
 
+__device__ const double k_unit_half[3] = {1, 1, 1}, k_zero_aabb[6] = {0, 0, 0, 0, 0, 0};
+
 // One object: place the model (or the object's own box) and take the bounds of the placed hull.  The placement is
-// scene_synthesis/utils.py:114-163 in its order: scale = size / raw_sizes, centroid = centre of the scaled raw AABB,
-// v * scale - centroid, then .dot(R) + t with R[0][0] = R[2][2] = cos, R[0][2] = -sin, R[2][0] = sin built from the
-// fp32 angle (np.cos of a float32 is a float32).  x and z are linear in (v.x, v.z), so their extremes over the mesh
-// lie on the xz convex hull; y needs only the raw y range.
+// make_placement (placement.cuh), shared with the renderer.  x and z are linear in (v.x, v.z), so their extremes over
+// the mesh lie on the xz convex hull; y needs only the raw y range.
 __global__ void k_scene_boxes(const float* __restrict__ trans, const float* __restrict__ size,
                               const float* __restrict__ angle, const int64_t* __restrict__ model, int Q,
                               const int* __restrict__ hull_off, const double* __restrict__ hull_xz, int H,
@@ -49,33 +50,27 @@ __global__ void k_scene_boxes(const float* __restrict__ trans, const float* __re
       return;
     }
   }
-  const double sx = size[q * 3 + 0], sy = size[q * 3 + 1], sz = size[q * 3 + 2];
-  const double tx = trans[q * 3 + 0], ty = trans[q * 3 + 1], tz = trans[q * 3 + 2];
-  // correctly rounded float32 cos / sin of the float32 angle, as numpy's float32 cos / sin give them
-  const double th = angle[q];
-  const double c = __double2float_rn(cos(th)), s = __double2float_rn(sin(th));
+  const bool own_box = beg == end;              // only the rotation and translation of p are used then
+  const Placement p = make_placement(size + q * 3, trans + q * 3, angle[q], own_box ? k_unit_half : raw_half + m * 3,
+                                     own_box ? k_zero_aabb : raw_aabb + m * 6);
   double ylo, yhi, x1 = INFINITY, x2 = -INFINITY, z1 = INFINITY, z2 = -INFINITY;
   auto put = [&](double px, double pz) {
-    const double x = __dadd_rn(__dadd_rn(__dmul_rn(px, c), __dmul_rn(pz, s)), tx);
-    const double z = __dadd_rn(__dadd_rn(__dmul_rn(px, -s), __dmul_rn(pz, c)), tz);
+    double x, z;
+    rotate_xz(p, px, pz, x, z);
     x1 = fmin(x1, x); x2 = fmax(x2, x);
     z1 = fmin(z1, z); z2 = fmax(z2, z);
   };
-  if (beg == end) {                             // no footprint: the object is its own box, centred, half sizes = size
-    ylo = __dadd_rn(-sy, ty);
-    yhi = __dadd_rn(sy, ty);
+  if (own_box) {                                // no footprint: the object is its own box, centred, half sizes = size
+    const double sx = size[q * 3 + 0], sy = size[q * 3 + 1], sz = size[q * 3 + 2];
+    ylo = __dadd_rn(-sy, p.ty);
+    yhi = __dadd_rn(sy, p.ty);
     put(-sx, -sz); put(-sx, sz); put(sx, -sz); put(sx, sz);
   } else {
-    const double* h = raw_half + m * 3;
     const double* bb = raw_aabb + m * 6;
-    const double kx = __ddiv_rn(sx, h[0]), ky = __ddiv_rn(sy, h[1]), kz = __ddiv_rn(sz, h[2]);
-    const double cx = __dmul_rn(__dadd_rn(__dmul_rn(bb[0], kx), __dmul_rn(bb[3], kx)), 0.5);
-    const double cy = __dmul_rn(__dadd_rn(__dmul_rn(bb[1], ky), __dmul_rn(bb[4], ky)), 0.5);
-    const double cz = __dmul_rn(__dadd_rn(__dmul_rn(bb[2], kz), __dmul_rn(bb[5], kz)), 0.5);
-    ylo = __dadd_rn(__dsub_rn(__dmul_rn(bb[1], ky), cy), ty);
-    yhi = __dadd_rn(__dsub_rn(__dmul_rn(bb[4], ky), cy), ty);
+    ylo = __dadd_rn(__dsub_rn(__dmul_rn(bb[1], p.ky), p.cy), p.ty);
+    yhi = __dadd_rn(__dsub_rn(__dmul_rn(bb[4], p.ky), p.cy), p.ty);
     for (int v = beg; v < end; ++v)
-      put(__dsub_rn(__dmul_rn(hull_xz[2 * v], kx), cx), __dsub_rn(__dmul_rn(hull_xz[2 * v + 1], kz), cz));
+      put(__dsub_rn(__dmul_rn(hull_xz[2 * v], p.kx), p.cx), __dsub_rn(__dmul_rn(hull_xz[2 * v + 1], p.kz), p.cz));
   }
   o[0] = x1; o[1] = fmin(ylo, yhi); o[2] = z1;  // a negative size mirrors the object: min <= max still holds
   o[3] = x2; o[4] = fmax(ylo, yhi); o[5] = z2;

@@ -141,13 +141,12 @@ def scene_stats(bounds: torch.Tensor, class_index: torch.Tensor, keep: Optional[
     return out
 
 
-def evaluate_samples(network, samples: torch.Tensor, bounds, catalog: Optional[ObjectCatalog] = None,
-                     mode: str = "objfeats", pair_iou: bool = False) -> Dict[str, torch.Tensor]:
-    """Scene statistics of a batch of network samples [B, N, d] on the device, with no per-scene host loop: the keep
-    mask of `delete_empty_batched`, `post_process_batch`, the class index (argmax over all class channels), retrieval
-    from `catalog` in `mode` ("objfeats", "objfeats_and_size" or "box"), the placed bounds and the statistics.
-    Without a catalogue every object is its own box and symmetry ignores models.  Returns STAT_KEYS plus "bounds",
-    "keep", "class_index" and "model_index" (None without a catalogue)."""
+def place_samples(network, samples: torch.Tensor, bounds, catalog: Optional[ObjectCatalog] = None,
+                  mode: str = "objfeats"):
+    """The placed objects of a batch of network samples [B, N, d] on the device: the keep mask of
+    `delete_empty_batched`, the class index (argmax over all class channels), the world-space attributes of
+    `post_process_batch` and the catalogue indices retrieved from `catalog` in `mode` ("objfeats",
+    "objfeats_and_size" or "box"; None without a catalogue) -> (world, keep, class_index, model_index)."""
     td, sd, bb, cd = network.translation_dim, network.size_dim, network.bbox_dim, network.class_dim
     keep = ~(samples[:, :, bb + cd - 1] >= 0)
     cls = samples[:, :, bb:bb + cd - 1].argmax(dim=-1)
@@ -159,9 +158,21 @@ def evaluate_samples(network, samples: torch.Tensor, bounds, catalog: Optional[O
         if "objfeats" not in bounds and "objfeats_32" in bounds:
             bounds = dict(bounds, objfeats=bounds["objfeats_32"])
     world = post_process_batch(params, bounds)
-    model_index = model_ids = None
+    model_index = None
     if catalog is not None:
         model_index = catalog.retrieve(cls, world.get("objfeats"), world["sizes"], mode)
+    return world, keep, cls, model_index
+
+
+def evaluate_samples(network, samples: torch.Tensor, bounds, catalog: Optional[ObjectCatalog] = None,
+                     mode: str = "objfeats", pair_iou: bool = False) -> Dict[str, torch.Tensor]:
+    """Scene statistics of a batch of network samples [B, N, d] on the device, with no per-scene host loop: the placed
+    objects of `place_samples`, their bounds and the statistics.  Without a catalogue every object is its own box and
+    symmetry ignores models.  Returns STAT_KEYS plus "bounds", "keep", "class_index" and "model_index" (None without a
+    catalogue)."""
+    world, keep, cls, model_index = place_samples(network, samples, bounds, catalog, mode)
+    model_ids = None
+    if catalog is not None:
         model_ids = torch.where(model_index >= 0, catalog.model_ids[model_index.clamp(min=0)], -1)
     boxes = scene_boxes(world["translations"], world["sizes"], world["angles"], model_index, catalog)
     out = scene_stats(boxes, cls, keep, model_ids, pair_iou=pair_iou)

@@ -335,6 +335,90 @@ DS_API int ds_scene_stats(const double* bounds_dev, const uint8_t* keep_dev, con
                           int32_t* num_pairs_dev, float* iou_sum_dev, int32_t* insec_count_dev,
                           float* overlap_ratio_dev, int32_t* num_symmetry_dev, float* pair_iou_dev, void* stream);
 
+/* ---- rendering: top-down images of placed scenes ------------------------------------------------
+ * The reference renders every scene top-down with simple-3dviz (scripts/utils.py:220-254); these calls draw the
+ * placed catalogue meshes of a whole batch of scenes straight into device memory (DESIGN.md, "Rendering").
+ *
+ * ds_mesh_catalog_create copies a mesh catalogue from HOST arrays to `device` and returns its handle:
+ * vertex_offsets / face_offsets [num_models + 1] int32 (both start at 0), vertices [V, 3] fp32 raw vertices, faces
+ * [F, 3] int32 model-local vertex indices, uvs [F, 3, 2] fp32 per-corner texture coordinates (NaN: the face has none),
+ * raw_half [num_models, 3] and raw_aabb [num_models, 6] fp64 as ds_scene_boxes takes them, kd [num_models, 3] fp32
+ * and textures [num_models, texture_size, texture_size, 3] uint8 (row 0 is the image's top row).  DS_ERR_INVALID for
+ * a NULL handle pointer or array, offsets that do not start at 0 or decrease, a face index outside its model, a model
+ * with 2^25 faces or more, a half size <= 0 or a texture size outside [1, 4096].  ds_mesh_catalog_destroy frees it;
+ * any pointer that is not a live catalogue handle gives DS_ERR_INVALID. */
+typedef struct ds_render_camera {
+  float eye[3], target[3], up[3];       /* pyrr create_look_at(eye, target, up) */
+  float left, right, bottom, top;       /* pyrr orthogonal_projection(left, right, bottom, top, near, far) */
+  float near_plane, far_plane;          /* 0 <= near < far: depth range kept per pixel */
+  int32_t width, height;                /* image size, each in [1, 4096] */
+  int32_t reserved[4];
+} ds_render_camera;
+
+enum { DS_RENDER_NO_TEXTURE = 1, DS_RENDER_WHITE_BACKGROUND = 2 };
+
+/* Per-call inputs of ds_render_scenes; every pointer is a device pointer.  Scene b holds num_objects slots
+ * (<= 64): translation / size [batch, num_objects, 3] and angle [batch, num_objects] fp32 in world space (after
+ * post_process_batch), model_index [batch, num_objects] int64 into the catalogue (-1: empty slot), class_index
+ * [batch, num_objects] int64 into palette [num_colors, 3] fp32 (needed with DS_RENDER_NO_TEXTURE only).  The optional
+ * floor of scene b is triangles floor_offsets[b] .. floor_offsets[b + 1] of floor_tris [num_floor_tris, 3, 3] fp32,
+ * already centred; floor_offsets NULL draws no floor.  floor_texture_index [batch] int32 (optional) picks one of
+ * floor_textures [num_floor_textures, S, S, 3] uint8 per scene (-1 or NULL: white).  Outputs: image [batch, height,
+ * width, 3] uint8 and, when id is not NULL, id [batch, height, width] int64 = slot << 32 | face of the visible
+ * triangle (slot num_objects: the floor), -1 for background. */
+typedef struct ds_render_args {
+  int32_t batch, num_objects;
+  const float* translation_dev;
+  const float* size_dev;
+  const float* angle_dev;
+  const int64_t* model_index_dev;
+  const int64_t* class_index_dev;
+  const int32_t* floor_offsets_dev;
+  const float* floor_tris_dev;
+  int32_t num_floor_tris;
+  int32_t num_colors;
+  const float* palette_dev;
+  const uint8_t* floor_textures_dev;
+  int32_t num_floor_textures, floor_texture_size;
+  const int32_t* floor_texture_index_dev;
+  int32_t flags;                        /* DS_RENDER_* */
+  int32_t reserved0;
+  uint8_t* image_dev;
+  int64_t* id_dev;
+  int32_t reserved[8];
+} ds_render_args;
+
+DS_API int ds_mesh_catalog_create(int32_t num_models, const int32_t* vertex_offsets, const float* vertices,
+                                  const int32_t* face_offsets, const int32_t* faces, const float* uvs,
+                                  const double* raw_half, const double* raw_aabb, const float* kd,
+                                  const uint8_t* textures, int32_t texture_size, int32_t device, void** handle);
+DS_API int ds_mesh_catalog_destroy(void* handle);
+/* Sample at pixel centres with a top-left fill rule and no culling; the nearest depth in [near, far] wins, ties go
+ * to the lower (slot, face).  DS_ERR_INVALID for a handle that is not a live catalogue or lives on another device,
+ * NULL required pointers, batch < 0, num_objects outside [0, 64], an unsupported image size or view volume, and
+ * (found on the device, so the call waits for `stream`) a model index outside [-1, M), a class index outside the
+ * palette, bad floor offsets or a floor texture index outside [-1, num_floor_textures). */
+DS_API int ds_render_scenes(void* handle, const ds_render_camera* camera, const ds_render_args* args, void* stream);
+
+/* Pillow's separable resize on the device, bit-exact with PIL given Pillow's coefficient tables (computed on the
+ * host by diffuscene_b200.render): horizontal pass, then vertical, with Pillow's intermediate rounding.  in [batch,
+ * in_h, in_w, 3] uint8.  Horizontal table: h_bounds [out_w, 2] int32 (first input column, count), h_coeffs
+ * [out_w, h_ksize]; vertical table likewise over rows.  Tables are device arrays.
+ * ds_resize_f32: each channel as a float32 'F' image, fp64 coefficients (clean-fid's clean resize), output
+ * [batch, 3, out_h, out_w] fp32 clipped to [0, 255].
+ * ds_resize_u8: 8-bit with int32 fixed-point coefficients (22 fraction bits), then (x / 255 - mean[c]) / std[c] in
+ * fp32 (ToTensor + Normalize; mean_std is a HOST array of 6 floats), output [batch, 3, out_h, out_w] fp32.
+ * DS_ERR_INVALID for NULL pointers, batch < 0, sizes outside [1, 4096], a kernel size outside [1, 1024] or a bound
+ * outside the input (found on the device, so these calls wait for `stream`). */
+DS_API int ds_resize_f32(const uint8_t* in_dev, int32_t batch, int32_t in_h, int32_t in_w, int32_t out_h,
+                         int32_t out_w, const int32_t* h_bounds_dev, const double* h_coeffs_dev, int32_t h_ksize,
+                         const int32_t* v_bounds_dev, const double* v_coeffs_dev, int32_t v_ksize, float* out_dev,
+                         void* stream);
+DS_API int ds_resize_u8(const uint8_t* in_dev, int32_t batch, int32_t in_h, int32_t in_w, int32_t out_h,
+                        int32_t out_w, const int32_t* h_bounds_dev, const int32_t* h_coeffs_dev, int32_t h_ksize,
+                        const int32_t* v_bounds_dev, const int32_t* v_coeffs_dev, int32_t v_ksize,
+                        const float* mean_std, float* out_dev, void* stream);
+
 /* ---- floor-plan encoder --------------------------------------------------------------------
  * Replaces the ResNet-18 trunk of the reference's room-mask feature extractor (scene_synthesis/networks/
  * feature_extractors.py:19-47 with FrozenBatchNorm2d, frozen_batchnorm.py): conv1 -> bn1 -> ReLU -> maxpool ->

@@ -13,6 +13,14 @@ generate_objautoencoder.py writes (latents, labels, sizes), optionally with the 
 `evaluate.footprint_table` (hull_offsets, hull_xz, raw_half, raw_aabb) and `model_ids`; without it every object is
 its own box.  With a retrieval mode other than "box" a second line per scene scores the size-retrieved models, as the
 reference's "retrive only size" line does.
+
+`--render_top2down` (opt-in) renders every scene top-down on the device with the reference's camera
+(diffuscene_b200.render) and writes `scene_XXXXX_render.png` next to its `.npz`, which then also holds the catalogue
+`model_index` of each object.  It needs `--mesh_catalogue` (scripts/pack_mesh_catalogue.py, in the order of
+`--catalogue`, which does the retrieval).  The samples carry no floor plan, so scenes render on a black background
+without a floor, or white with `--without_floor`; render the real scenes the same way (scripts/render_scenes.py).
+The shading is this project's: FID / KID / precision-recall of these images compare only with native renders of the
+real scenes, never with the reference's simple-3dviz images.
 """
 import argparse
 import os
@@ -60,7 +68,15 @@ def main(argv):
     p.add_argument("--catalogue", default=None, help="catalogue.npz of the models to place (default: boxes)")
     p.add_argument("--retrieve_mode", default=None, choices=["objfeats", "objfeats_and_size", "box"],
                    help="retrieval for --compute_intersec (default: objfeats when the network and catalogue have them)")
+    p.add_argument("--render_top2down", action="store_true",
+                   help="write scene_XXXXX_render.png top-down renders (native shading: compare only with native "
+                        "renders of the real scenes, scripts/render_scenes.py)")
+    p.add_argument("--mesh_catalogue", default=None, help="mesh_catalogue.npz for --render_top2down")
+    p.add_argument("--no_texture", action="store_true", help="--render_top2down with flat per-class colours")
+    p.add_argument("--without_floor", action="store_true", help="--render_top2down on a white background")
     args = p.parse_args(argv)
+    if args.render_top2down and (args.mesh_catalogue is None or args.catalogue is None):
+        p.error("--render_top2down needs --mesh_catalogue and the --catalogue that retrieves from it")
     if not torch.cuda.is_available():
         raise RuntimeError("generate_diffusion.py needs a CUDA device (H100); there is no CPU path")
     device = torch.device("cuda:0")
@@ -80,6 +96,16 @@ def main(argv):
         if catalog is not None and mode != "box":
             aggs.append(PlausibilityAggregator(PlausibilityAggregator.SUFFIX_ONLYSIZE))
             modes.append("box")
+    if args.render_top2down:
+        from diffuscene_b200.evaluate import place_samples
+        from diffuscene_b200.render import MeshCatalog, hls_palette, render_scenes
+        from PIL import Image
+        render_cat, render_mode = _catalogue(args.catalogue, network, args.retrieve_mode)
+        meshes = MeshCatalog(args.mesh_catalogue)
+        if meshes.num_models != len(render_cat.model_ids):
+            raise ValueError("the mesh catalogue holds %d models, the retrieval catalogue %d"
+                             % (meshes.num_models, len(render_cat.model_ids)))
+        palette = hls_palette(network.class_dim - 1)
     done = 0
     while done < args.n_sequences:
         bs = min(args.batch_size, args.n_sequences - done)
@@ -90,11 +116,22 @@ def main(argv):
             room_mask = torch.zeros(bs, 1, 64, 64, device=device)
         samples = network.sample(room_mask, N, d, batch_size=bs, clip_denoised=args.clip_denoised, ddim=args.ddim,
                                  ddim_steps=args.ddim_steps, seed=args.seed * 100003 + done)
+        if args.render_top2down:
+            world, keep, cls, model_index = place_samples(network, samples, ds.bounds, render_cat, render_mode)
+            model_index = torch.where(keep, model_index, -1)
+            images = render_scenes(meshes, world["translations"], world["sizes"], world["angles"], model_index, cls,
+                                   no_texture=args.no_texture, white_background=args.without_floor,
+                                   palette=palette).cpu().numpy()
+            kept_models = [model_index[b][keep[b]].cpu().numpy() for b in range(bs)]
         for i, scene in enumerate(network.delete_empty_batched(samples)):
             boxes = {k: v[None].numpy() for k, v in scene.items() if k != "class_index"}
             out = ds.post_process(boxes)
             out["class_index"] = scene["class_index"].numpy()
-            np.savez(os.path.join(args.output_directory, "scene_{:05d}.npz".format(done + i)), **out)
+            name = os.path.join(args.output_directory, "scene_{:05d}".format(done + i))
+            if args.render_top2down:
+                out["model_index"] = kept_models[i]
+                Image.fromarray(images[i]).save(name + "_render.png")
+            np.savez(name + ".npz", **out)
         if args.compute_intersec:
             lines = [agg.update(evaluate_samples(network, samples, ds.bounds, catalog, m)) for agg, m in zip(aggs, modes)]
             with open(os.path.join(args.output_directory, "iou_states.txt"), "a") as f:
