@@ -72,7 +72,7 @@ class DsInceptionConfig(C.Structure):
 class DsRenderCamera(C.Structure):
     _fields_ = [("eye", C.c_float * 3), ("target", C.c_float * 3), ("up", C.c_float * 3)] + \
         [(n, C.c_float) for n in ("left", "right", "bottom", "top", "near_plane", "far_plane")] + \
-        [("width", C.c_int32), ("height", C.c_int32), ("reserved", C.c_int32 * 4)]
+        [("width", C.c_int32), ("height", C.c_int32), ("projection", C.c_int32), ("reserved", C.c_int32 * 3)]
 
 
 class DsRenderArgs(C.Structure):
@@ -86,6 +86,7 @@ class DsRenderArgs(C.Structure):
 
 
 DS_RENDER_NO_TEXTURE, DS_RENDER_WHITE_BACKGROUND = 1, 2
+DS_RENDER_ORTHOGRAPHIC, DS_RENDER_PERSPECTIVE = 0, 1
 
 
 class DsVlbArgs(C.Structure):

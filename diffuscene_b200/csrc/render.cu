@@ -1,13 +1,17 @@
 // Top-down rendering of placed furniture meshes (the reference's render_top2down through simple-3dviz,
-// scripts/generate_diffusion.py:251-264 / preprocess_data.py:297-350): a batched orthographic rasterizer writing
-// uint8 [B, H, W, 3] images on the device.  Stateful catalogue handle (ds_mesh_catalog_*) and one render call.
+// scripts/generate_diffusion.py:251-264 / preprocess_data.py:297-350) and the perspective views of its
+// completion / rearrangement driver (scripts/utils.py:431-458): a batched rasterizer writing uint8 [B, H, W, 3]
+// images on the device.  Stateful catalogue handle (ds_mesh_catalog_*) and one render call.
 //
-// Pipeline per call:
+// Pipeline per call (both kernels are templated on the projection; the orthographic instantiation is the original):
 //   k_render_prep    one thread per (scene, slot): the shared placement (placement.cuh) composed with the camera into
-//                    fp32 affine maps raw vertex -> (pixel x, pixel y, depth) and raw vertex -> world, and the
-//                    object's conservative pixel bounds; slot N is the scene's floor.
+//                    fp32 affine maps raw vertex -> (pixel x, pixel y, depth) (perspective: (pixel x * depth,
+//                    pixel y * depth, depth), divided per vertex) and raw vertex -> world, and the object's
+//                    conservative pixel bounds; slot N is the scene's floor.
 //   k_render_tiles   one CTA per (scene, 64 x 64 tile): visibility by atomicMin of (depth bits, slot, face) into a
 //                    shared-memory tile, then a resolve pass per pixel that recomputes barycentrics and shades.
+//                    Perspective faces are clipped at depth = near in view space into at most two triangles first;
+//                    depth and barycentrics are interpolated perspective-correctly.
 // atomicMin is order independent, so an image depends neither on scheduling nor on the rest of the batch.
 #include <mutex>
 #include <set>
@@ -78,6 +82,7 @@ __device__ void compose(const Cam& cam, const Placement& p, float (*px)[4], floa
   }
 }
 
+template <bool PERSP>
 __global__ void k_render_prep(Cam cam, const float* __restrict__ trans, const float* __restrict__ size,
                               const float* __restrict__ angle, const int64_t* __restrict__ model,
                               const int64_t* __restrict__ cls, int num_colors, int check_cls,
@@ -136,6 +141,42 @@ __global__ void k_render_prep(Cam cam, const float* __restrict__ trans, const fl
         }
       }
     o.umin = umin; o.vmin = vmin;
+  }
+  if constexpr (PERSP) {
+    // rows 0 and 1 are pixel coordinates times depth: the pixel range of a box wholly in front of the near plane is
+    // that of its divided corners (a projective map keeps convex hulls there); a box that reaches the near plane
+    // may cover any pixel
+    if (o.faces > 0 && hi[2] >= cam.near_p * 0.999f && lo[2] <= cam.far_p * 1.001f) {
+      if (lo[2] >= cam.near_p * 1.001f) {
+        float sl[2] = {INFINITY, INFINITY}, sh[2] = {-INFINITY, -INFINITY};
+        if (slot < N) {
+          const double* bb = aabb + model[(int64_t)b * N + slot] * 6;
+          for (int c = 0; c < 8; ++c) {
+            const float vx = (float)bb[(c & 1) ? 3 : 0], vy = (float)bb[(c & 2) ? 4 : 1], vz = (float)bb[(c & 4) ? 5 : 2];
+            const float d = apply(o.m[2], vx, vy, vz);
+            for (int r = 0; r < 2; ++r) {
+              const float v = __fdiv_rn(apply(o.m[r], vx, vy, vz), d);
+              sl[r] = fminf(sl[r], v); sh[r] = fmaxf(sh[r], v);
+            }
+          }
+        } else {
+          for (int t = floor_off[b]; t < floor_off[b + 1]; ++t)
+            for (int k = 0; k < 3; ++k) {
+              const float* v = floor_tris + (int64_t)t * 9 + k * 3;
+              const float d = apply(o.m[2], v[0], v[1], v[2]);
+              for (int r = 0; r < 2; ++r) {
+                const float s = __fdiv_rn(apply(o.m[r], v[0], v[1], v[2]), d);
+                sl[r] = fminf(sl[r], s); sh[r] = fmaxf(sh[r], s);
+              }
+            }
+        }
+        lo[0] = sl[0]; hi[0] = sh[0]; lo[1] = sl[1]; hi[1] = sh[1];
+      } else {
+        lo[0] = lo[1] = -INFINITY; hi[0] = hi[1] = INFINITY;
+      }
+    } else {
+      lo[0] = 1.f; hi[0] = 0.f;                    // culled
+    }
   }
   // conservative pixel range (one pixel of slack for the fp32 rounding of the composed map), depth culled only when
   // the whole box lies beyond the clip range
@@ -219,6 +260,78 @@ __device__ __forceinline__ void sample_rgb(const uint8_t* tex, int T, float u, f
 
 struct BigTri { Tri t; int face, x0, y0, x1, y1; };
 
+// Point of edge a -> b (a in front of the near plane, b behind) at depth = near, from the homogeneous (X, Y, depth)
+// corners.  The front endpoint always comes first, so two faces sharing the edge get the same bits (watertight).
+__device__ __forceinline__ void clip_point(const float* X, const float* Y, const float* D, int a, int b, float near,
+                                           float& x, float& y) {
+  const float t = __fdiv_rn(__fsub_rn(near, D[a]), __fsub_rn(D[b], D[a]));
+  x = __fdiv_rn(__fadd_rn(X[a], __fmul_rn(t, __fsub_rn(X[b], X[a]))), near);
+  y = __fdiv_rn(__fadd_rn(Y[a], __fmul_rn(t, __fsub_rn(Y[b], Y[a]))), near);
+}
+
+// The part of a face with view depth >= near as at most two screen triangles whose d[] holds 1 / depth; both keep
+// the face's winding.  Returns their count.
+__device__ __forceinline__ int clip_near(const float* X, const float* Y, const float* D, float near, Tri* out) {
+  const float rn = __frcp_rn(near);
+  int nin = 0, i_in = 0, i_out = 0;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    if (D[k] >= near) { ++nin; i_in = k; } else { i_out = k; }
+  }
+  if (nin == 0) return 0;
+  if (nin == 3) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      out[0].x[k] = __fdiv_rn(X[k], D[k]); out[0].y[k] = __fdiv_rn(Y[k], D[k]); out[0].d[k] = __frcp_rn(D[k]);
+    }
+    return 1;
+  }
+  if (nin == 1) {                                   // (i, i -> j at near, i -> k at near)
+    const int i = i_in, j = (i + 1) % 3, k = (i + 2) % 3;
+    out[0].x[0] = __fdiv_rn(X[i], D[i]); out[0].y[0] = __fdiv_rn(Y[i], D[i]); out[0].d[0] = __frcp_rn(D[i]);
+    clip_point(X, Y, D, i, j, near, out[0].x[1], out[0].y[1]);
+    clip_point(X, Y, D, i, k, near, out[0].x[2], out[0].y[2]);
+    out[0].d[1] = out[0].d[2] = rn;
+    return 1;
+  }
+  // two in front (i, j), k behind: the quad (i, j, j -> k, i -> k) as (i, j, p) and (i, p, q)
+  const int k = i_out, i = (k + 1) % 3, j = (k + 2) % 3;
+  float px, py, qx, qy;
+  clip_point(X, Y, D, j, k, near, px, py);
+  clip_point(X, Y, D, i, k, near, qx, qy);
+  const float xi = __fdiv_rn(X[i], D[i]), yi = __fdiv_rn(Y[i], D[i]), ri = __frcp_rn(D[i]);
+  out[0].x[0] = xi; out[0].y[0] = yi; out[0].d[0] = ri;
+  out[0].x[1] = __fdiv_rn(X[j], D[j]); out[0].y[1] = __fdiv_rn(Y[j], D[j]); out[0].d[1] = __frcp_rn(D[j]);
+  out[0].x[2] = px; out[0].y[2] = py; out[0].d[2] = rn;
+  out[1].x[0] = xi; out[1].y[0] = yi; out[1].d[0] = ri;
+  out[1].x[1] = px; out[1].y[1] = py; out[1].d[1] = rn;
+  out[1].x[2] = qx; out[1].y[2] = qy; out[1].d[2] = rn;
+  return 2;
+}
+
+// Perspective-correct barycentrics of pixel centre (px, py) on the plane of a face with homogeneous corners
+// (X, Y, depth): w_k is proportional to the 2-D cross product of corners k + 1 and k + 2 taken relative to the pixel's
+// ray, which needs no clipping.
+__device__ __forceinline__ void persp_bary(const float* X, const float* Y, const float* D, float px, float py,
+                                           float* w) {
+  float rx[3], ry[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    rx[k] = __fsub_rn(X[k], __fmul_rn(px, D[k]));
+    ry[k] = __fsub_rn(Y[k], __fmul_rn(py, D[k]));
+  }
+  float e[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const int a = (k + 1) % 3, b = (k + 2) % 3;
+    e[k] = __fsub_rn(__fmul_rn(rx[a], ry[b]), __fmul_rn(ry[a], rx[b]));
+  }
+  const float s = __fadd_rn(__fadd_rn(e[0], e[1]), e[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) w[k] = s != 0.f ? __fdiv_rn(e[k], s) : 1.f / 3.f;
+}
+
+template <bool PERSP>
 __global__ void __launch_bounds__(RT_THREADS)
 k_render_tiles(Cam cam, const ObjXf* __restrict__ xf, const int64_t* __restrict__ model,
                const int64_t* __restrict__ cls, const float* __restrict__ palette, int flags,
@@ -241,7 +354,8 @@ k_render_tiles(Cam cam, const ObjXf* __restrict__ xf, const int64_t* __restrict_
   auto plot = [&](const Tri& t, unsigned id, int x, int y) {
     float w[3];
     if (!cover(t, __fadd_rn((float)x, 0.5f), __fadd_rn((float)y, 0.5f), w)) return;
-    const float d = interp(t.d, w);
+    float d = interp(t.d, w);
+    if constexpr (PERSP) d = __fdiv_rn(1.f, d);          // t.d holds 1 / depth, linear in screen space
     if (!(d >= cam.near_p && d <= cam.far_p)) return;   // per-pixel near / far clipping; NaN is never drawn
     const unsigned long long key = ((unsigned long long)__float_as_uint(fmaxf(d, 0.f)) << 32) | id;
     atomicMin(&s_key[(y - ty0) * RT + (x - tx0)], key);
@@ -256,35 +370,56 @@ k_render_tiles(Cam cam, const ObjXf* __restrict__ xf, const int64_t* __restrict_
     for (int f0 = 0; f0 < nf; f0 += RT_THREADS) {
       const int f = f0 + threadIdx.x;
       if (f < nf) {
-        Tri t;
-        float lx = INFINITY, hx = -INFINITY, ly = INFINITY, hy = -INFINITY;
+        const unsigned id = ((unsigned)slot << FACE_BITS) | (unsigned)f;
+        auto emit = [&](const Tri& t) {
+          float lx = INFINITY, hx = -INFINITY, ly = INFINITY, hy = -INFINITY;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            lx = fminf(lx, t.x[k]); hx = fmaxf(hx, t.x[k]); ly = fminf(ly, t.y[k]); hy = fmaxf(hy, t.y[k]);
+          }
+          // pixels whose centres can lie in the triangle, clipped to the tile
+          const int x0 = (int)fmaxf((float)tx0, ceilf(__fsub_rn(lx, 0.5f)));
+          const int x1 = (int)fminf((float)tx1, floorf(__fsub_rn(hx, 0.5f)));
+          const int y0 = (int)fmaxf((float)ty0, ceilf(__fsub_rn(ly, 0.5f)));
+          const int y1 = (int)fminf((float)ty1, floorf(__fsub_rn(hy, 0.5f)));
+          if (x0 <= x1 && y0 <= y1) {
+            if ((x1 - x0 + 1) * (y1 - y0 + 1) <= SMALL_TRI_PIXELS) {
+              for (int y = y0; y <= y1; ++y)
+                for (int x = x0; x <= x1; ++x) plot(t, id, x, y);
+            } else {
+              const int q = atomicAdd(&s_nbig, 1);
+              if (q < RT_THREADS) {
+                s_big[q] = BigTri{t, f, x0, y0, x1, y1};
+              } else {                              // a clipped face's second half found the list full
+                for (int y = y0; y <= y1; ++y)
+                  for (int x = x0; x <= x1; ++x) plot(t, id, x, y);
+              }
+            }
+          }
+        };
+        float X[3], Y[3], D[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
           float vx, vy, vz;
           corner(slot, N, f, k, faces, face_off, vert_off, verts, m, floor_tris, fbeg, vx, vy, vz);
-          t.x[k] = apply(o.m[0], vx, vy, vz);
-          t.y[k] = apply(o.m[1], vx, vy, vz);
-          t.d[k] = apply(o.m[2], vx, vy, vz);
-          lx = fminf(lx, t.x[k]); hx = fmaxf(hx, t.x[k]); ly = fminf(ly, t.y[k]); hy = fmaxf(hy, t.y[k]);
+          X[k] = apply(o.m[0], vx, vy, vz);
+          Y[k] = apply(o.m[1], vx, vy, vz);
+          D[k] = apply(o.m[2], vx, vy, vz);
         }
-        // pixels whose centres can lie in the triangle, clipped to the tile
-        const int x0 = (int)fmaxf((float)tx0, ceilf(__fsub_rn(lx, 0.5f)));
-        const int x1 = (int)fminf((float)tx1, floorf(__fsub_rn(hx, 0.5f)));
-        const int y0 = (int)fmaxf((float)ty0, ceilf(__fsub_rn(ly, 0.5f)));
-        const int y1 = (int)fminf((float)ty1, floorf(__fsub_rn(hy, 0.5f)));
-        const unsigned id = ((unsigned)slot << FACE_BITS) | (unsigned)f;
-        if (x0 <= x1 && y0 <= y1) {
-          if ((x1 - x0 + 1) * (y1 - y0 + 1) <= SMALL_TRI_PIXELS) {
-            for (int y = y0; y <= y1; ++y)
-              for (int x = x0; x <= x1; ++x) plot(t, id, x, y);
-          } else {
-            const int q = atomicAdd(&s_nbig, 1);
-            s_big[q] = BigTri{t, f, x0, y0, x1, y1};
-          }
+        if constexpr (PERSP) {
+          Tri sub[2];
+          const int ns = clip_near(X, Y, D, cam.near_p, sub);
+          if (ns > 0) emit(sub[0]);
+          if (ns > 1) emit(sub[1]);
+        } else {
+          Tri t;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) { t.x[k] = X[k]; t.y[k] = Y[k]; t.d[k] = D[k]; }
+          emit(t);
         }
       }
       __syncthreads();
-      const int nbig = s_nbig;
+      const int nbig = min(s_nbig, RT_THREADS);
       for (int q = 0; q < nbig; ++q) {              // large triangles: the CTA splits their pixels
         const BigTri& bt = s_big[q];
         const int w = bt.x1 - bt.x0 + 1, n = w * (bt.y1 - bt.y0 + 1);
@@ -324,7 +459,10 @@ k_render_tiles(Cam cam, const ObjXf* __restrict__ xf, const int64_t* __restrict_
         for (int r = 0; r < 3; ++r) wv[r][k] = apply(o.m[3 + r], vx, vy, vz);
       }
       float w[3];
-      cover(t, __fadd_rn((float)x, 0.5f), __fadd_rn((float)y, 0.5f), w);
+      if constexpr (PERSP)
+        persp_bary(t.x, t.y, t.d, __fadd_rn((float)x, 0.5f), __fadd_rn((float)y, 0.5f), w);
+      else
+        cover(t, __fadd_rn((float)x, 0.5f), __fadd_rn((float)y, 0.5f), w);
       float base[3] = {1.f, 1.f, 1.f};
       if (slot < N) {
         if (flags & RF_NO_TEXTURE) {
@@ -479,9 +617,14 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
   if (camera->width < 1 || camera->width > 4096 || camera->height < 1 || camera->height > 4096)
     return fail(DS_ERR_INVALID, "ds_render_scenes: image size %d x %d outside [1, 4096]", camera->width,
                 camera->height);
+  const int proj = camera->projection;
+  if (proj != DS_RENDER_ORTHOGRAPHIC && proj != DS_RENDER_PERSPECTIVE)
+    return fail(DS_ERR_INVALID, "ds_render_scenes: unknown projection %d", proj);
   if (!(camera->near_plane >= 0.f) || !(camera->far_plane > camera->near_plane) || camera->left == camera->right ||
       camera->bottom == camera->top)
     return fail(DS_ERR_INVALID, "ds_render_scenes: need 0 <= near < far and a non-empty view volume");
+  if (proj == DS_RENDER_PERSPECTIVE && !(camera->near_plane > 0.f))
+    return fail(DS_ERR_INVALID, "ds_render_scenes: a perspective view volume needs near > 0");
   if (!a->image_dev) return fail(DS_ERR_INVALID, "ds_render_scenes: NULL image pointer");
   if (a->num_objects > 0 && a->batch > 0 &&
       (!a->translation_dev || !a->size_dev || !a->angle_dev || !a->model_index_dev))
@@ -504,7 +647,8 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
                 c->device, cur);
   if (a->batch == 0) return 0;
 
-  // camera: pyrr's create_look_at and orthogonal_projection, then the viewport (DESIGN.md, rendering)
+  // camera: pyrr's create_look_at and orthogonal_projection (or create_perspective_projection_from_bounds), then the
+  // viewport (DESIGN.md, rendering)
   Cam cam;
   double e[3], f[3], u[3], sd[3];
   for (int k = 0; k < 3; ++k) { e[k] = camera->eye[k]; f[k] = (double)camera->target[k] - e[k]; u[k] = camera->up[k]; }
@@ -531,6 +675,19 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
   cam.m[0][3] = ox - sx * (sd[0] * e[0] + sd[1] * e[1] + sd[2] * e[2]);
   cam.m[1][3] = oy - sy * (up2[0] * e[0] + up2[1] * e[1] + up2[2] * e[2]);
   cam.m[2][3] = -(f[0] * e[0] + f[1] * e[1] + f[2] * e[2]);
+  if (proj == DS_RENDER_PERSPECTIVE) {
+    // clip x = 2 n / (R - L) x_view - (R + L) / (R - L) depth with w = depth, so pixel x * depth = W / 2 (clip x +
+    // depth) is affine in the vertex; likewise pixel y * depth
+    const double n = camera->near_plane;
+    const double px = W * n / (R - L), pd = W / 2 * (1.0 - (R + L) / (R - L));
+    const double qy = H * n / (To - Bo), qd = H / 2 * (1.0 - (To + Bo) / (To - Bo));
+    for (int c = 0; c < 4; ++c) {
+      const double vx = c < 3 ? sd[c] : -(sd[0] * e[0] + sd[1] * e[1] + sd[2] * e[2]);
+      const double vy = c < 3 ? up2[c] : -(up2[0] * e[0] + up2[1] * e[1] + up2[2] * e[2]);
+      cam.m[0][c] = px * vx + pd * cam.m[2][c];
+      cam.m[1][c] = qy * vy + qd * cam.m[2][c];
+    }
+  }
   cam.near_p = camera->near_plane;
   cam.far_p = camera->far_plane;
   for (int k = 0; k < 3; ++k) cam.eye[k] = camera->eye[k];
@@ -544,14 +701,15 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
   CK(cudaMallocAsync(&xf, sizeof(ObjXf) * (int64_t)B * (N + 1), s));
   CK(cudaMallocAsync(&err_dev, sizeof(int), s));
   CK(cudaMemsetAsync(err_dev, 0, sizeof(int), s));
-  k_render_prep<<<cdiv((int64_t)B * (N + 1), 128), 128, 0, s>>>(
+  const bool persp = proj == DS_RENDER_PERSPECTIVE;
+  (persp ? k_render_prep<true> : k_render_prep<false>)<<<cdiv((int64_t)B * (N + 1), 128), 128, 0, s>>>(
       cam, a->translation_dev, a->size_dev, a->angle_dev, a->model_index_dev, a->class_index_dev, a->num_colors,
       no_tex, c->vert_off, c->verts, c->face_off, c->half, c->aabb, c->M, a->floor_offsets_dev, a->floor_tris_dev,
       a->num_floor_tris, a->floor_texture_index_dev, a->num_floor_textures, B, N, xf, err_dev);
   cudaError_t ce = cudaGetLastError();
   const int tiles_x = cdiv(cam.W, RT), tiles_y = cdiv(cam.H, RT);
   if (ce == cudaSuccess) {
-    k_render_tiles<<<dim3(tiles_x * tiles_y, B), RT_THREADS, 0, s>>>(
+    (persp ? k_render_tiles<true> : k_render_tiles<false>)<<<dim3(tiles_x * tiles_y, B), RT_THREADS, 0, s>>>(
         cam, xf, a->model_index_dev, a->class_index_dev, a->palette_dev, a->flags, c->vert_off, c->verts, c->face_off,
         c->faces, c->uvs, c->kd, c->tex, c->T, a->floor_offsets_dev, a->floor_tris_dev, a->floor_textures_dev,
         a->floor_texture_index_dev, a->floor_texture_size, N, tiles_x, (uint8_t*)a->image_dev, (int64_t*)a->id_dev);

@@ -52,6 +52,28 @@ def encode_batch(params: Mapping[str, torch.Tensor], bounds: Mapping[str, Sequen
     return out
 
 
+def load_dataset_stats(path: str) -> Dict[str, tuple]:
+    """`bounds` for encode_batch / post_process_batch from the reference's dataset_stats.txt JSON: bounds_translations
+    / bounds_sizes are 6 floats (lo xyz, hi xyz), bounds_angles 2 (lo, hi), bounds_objfeats[_32] 3 (std, lo, hi)."""
+    import json
+
+    import numpy as np
+    with open(path) as f:
+        stats = json.load(f)
+    out: Dict[str, tuple] = {}
+    for key, n in (("translations", 6), ("sizes", 6), ("angles", 2), ("objfeats", 3), ("objfeats_32", 3)):
+        if "bounds_" + key not in stats:
+            continue
+        v = np.asarray(stats["bounds_" + key], np.float32).reshape(-1)
+        if v.size != n:
+            raise ValueError("%s: bounds_%s holds %d values, expected %d" % (path, key, v.size, n))
+        out[key] = tuple(np.split(v, n // (3 if n == 6 else 1)))
+    missing = [k for k in ("translations", "sizes", "angles") if k not in out]
+    if missing:
+        raise ValueError("%s lacks bounds_%s" % (path, ", bounds_".join(missing)))
+    return out
+
+
 def post_process_batch(params: Mapping[str, torch.Tensor], bounds: Mapping[str, Sequence]) -> Dict[str, torch.Tensor]:
     """Network-space samples -> world-space attributes for a whole batch (reference `post_process` :515-535)."""
     out: Dict[str, torch.Tensor] = {}

@@ -1,4 +1,4 @@
-"""Top-down rendering of scenes on the device, and renders fed to FID / KID and precision-recall without the host.
+"""Top-down and perspective rendering of scenes on the device, and renders fed to FID / KID and precision-recall without the host.
 
 The reference renders every scene top-down with simple-3dviz / OpenGL (scripts/utils.py:220-254,
 scripts/generate_diffusion.py:251-264, scripts/preprocess_data.py:297-350).  Here:
@@ -6,7 +6,8 @@ scripts/generate_diffusion.py:251-264, scripts/preprocess_data.py:297-350).  Her
   * `pack_catalogue` / `parse_obj` turn 3D-FUTURE model directories into one `mesh_catalogue.npz`, and
     `MeshCatalog` uploads it once (ds_mesh_catalog_*);
   * `render_scenes` rasterises the placed catalogue meshes (and the floor) of a whole batch of scenes into uint8
-    [B, H, W, 3] device images with the reference's orthographic top-down camera (ds_render_scenes);
+    [B, H, W, 3] device images with the reference's orthographic top-down camera or its perspective view
+    (REFERENCE_PERSPECTIVE) (ds_render_scenes);
   * `clean_resize` / `ipr_resize` are Pillow's resizes of the two metrics on the device, bit-exact with PIL
     (ds_resize_f32 / ds_resize_u8), from the coefficient tables `pillow_coeffs` computes on the host;
   * `inception_features` / `vgg16_features` / `evaluate_renders` take device renders to features and metrics.
@@ -201,10 +202,17 @@ class MeshCatalog:
 
 # ---- camera, palette, floors ------------------------------------------------------------------------------------
 
+PROJECTIONS = {"orthographic": capi.DS_RENDER_ORTHOGRAPHIC, "perspective": capi.DS_RENDER_PERSPECTIVE}
+
+
 @dataclass
 class Camera:
     """The reference's top-down camera (generate_diffusion.py:251-264): eye (0, 4, 0) looking at the origin with up
-    (0, 0, -1), Matrix44.orthogonal_projection(left=-s, right=s, bottom=s, top=-s, near=0.1, far=6), s = 3.1, 256^2."""
+    (0, 0, -1), Matrix44.orthogonal_projection(left=-s, right=s, bottom=s, top=-s, near=0.1, far=6), s = 3.1, 256^2.
+
+    With projection "perspective", left / right / bottom / top are the frustum bounds on the near plane (pyrr's
+    create_perspective_projection_from_bounds) and depth is the view depth -z_view; `Camera.perspective` builds one
+    from a vertical field of view."""
     eye: Tuple[float, float, float] = (0.0, 4.0, 0.0)
     target: Tuple[float, float, float] = (0.0, 0.0, 0.0)
     up: Tuple[float, float, float] = (0.0, 0.0, -1.0)
@@ -216,13 +224,38 @@ class Camera:
     far: float = 6.0
     width: int = 256
     height: int = 256
+    projection: str = "orthographic"
+
+    @classmethod
+    def perspective(cls, eye, target=(0.0, 0.0, 0.0), up=(0.0, 1.0, 0.0), fovy: float = 45.0, width: int = 512,
+                    height: int = 512, near: float = 0.1, far: float = 1000.0) -> "Camera":
+        """A perspective camera with pyrr's perspective_projection(fovy, width / height, near, far) bounds: ymax =
+        near tan(fovy pi / 360), xmax = ymax width / height.  bottom = ymax, top = -ymax keeps the image upright
+        (array row 0 is the top of the view), as the top-down camera's swapped bounds do.
+
+        45 degrees, 0.1 and 1000 are, as far as we know, simple-3dviz Scene's default projection, which the
+        reference's perspective renders use; simple-3dviz is not available to check this, and the shading is this
+        project's own either way."""
+        ymax = near * math.tan(fovy * math.pi / 360.0)
+        xmax = ymax * width / height
+        return cls(eye=tuple(float(v) for v in eye), target=tuple(float(v) for v in target),
+                   up=tuple(float(v) for v in up), left=-xmax, right=xmax, bottom=ymax, top=-ymax, near=near,
+                   far=far, width=width, height=height, projection="perspective")
 
     def struct(self) -> capi.DsRenderCamera:
+        if self.projection not in PROJECTIONS:
+            raise ValueError("unknown projection %r (one of %s)" % (self.projection, ", ".join(PROJECTIONS)))
         c = capi.DsRenderCamera()
         c.eye[:], c.target[:], c.up[:] = self.eye, self.target, self.up
         c.left, c.right, c.bottom, c.top = self.left, self.right, self.bottom, self.top
         c.near_plane, c.far_plane, c.width, c.height = self.near, self.far, self.width, self.height
+        c.projection = PROJECTIONS[self.projection]
         return c
+
+
+# the reference driver's perspective view (scripts/completion_rearrange.py defaults, scripts/utils.py:431-458)
+REFERENCE_PERSPECTIVE = Camera.perspective(eye=(-0.10923499, 1.9325259, -7.19009), target=(0.0, 0.0, 0.0),
+                                           up=(0.0, 1.0, 0.0), width=512, height=512)
 
 
 def hls_palette(n_colors: int, h: float = 0.01, l: float = 0.6, s: float = 0.65) -> np.ndarray:
@@ -274,7 +307,7 @@ def render_scenes(catalog: MeshCatalog, translations, sizes, angles, model_index
                   floors: Optional[Tuple[np.ndarray, np.ndarray]] = None, no_texture: bool = False,
                   white_background: bool = False, camera: Optional[Camera] = None, palette=None,
                   floor_textures=None, floor_texture_index=None, return_ids: bool = False):
-    """uint8 [B, H, W, 3] top-down renders on the catalogue's device.
+    """uint8 [B, H, W, 3] renders on the catalogue's device (top-down unless `camera` says otherwise).
 
     translations / sizes [B, N, 3] and angles [B, N] or [B, N, 1] are world-space (after post_process_batch);
     model_index [B, N] indexes the catalogue (-1: empty slot); class_index [B, N] picks the flat colour of each object

@@ -349,12 +349,19 @@ DS_API int ds_scene_stats(const double* bounds_dev, const uint8_t* keep_dev, con
  * any pointer that is not a live catalogue handle gives DS_ERR_INVALID. */
 typedef struct ds_render_camera {
   float eye[3], target[3], up[3];       /* pyrr create_look_at(eye, target, up) */
-  float left, right, bottom, top;       /* pyrr orthogonal_projection(left, right, bottom, top, near, far) */
-  float near_plane, far_plane;          /* 0 <= near < far: depth range kept per pixel */
+  float left, right, bottom, top;       /* orthographic: pyrr orthogonal_projection(left, right, bottom, top, near,
+                                           far); perspective: the frustum bounds on the near plane, pyrr
+                                           create_perspective_projection_from_bounds(left, right, bottom, top, near,
+                                           far).  Array row r counts from y_ndc = -1 in both: bottom > top gives an
+                                           upright image */
+  float near_plane, far_plane;          /* view depth (-z_view) range kept per pixel: 0 <= near < far, and near > 0
+                                           for perspective */
   int32_t width, height;                /* image size, each in [1, 4096] */
-  int32_t reserved[4];
+  int32_t projection;                   /* DS_RENDER_ORTHOGRAPHIC (0, a zeroed struct) or DS_RENDER_PERSPECTIVE */
+  int32_t reserved[3];
 } ds_render_camera;
 
+enum { DS_RENDER_ORTHOGRAPHIC = 0, DS_RENDER_PERSPECTIVE = 1 };
 enum { DS_RENDER_NO_TEXTURE = 1, DS_RENDER_WHITE_BACKGROUND = 2 };
 
 /* Per-call inputs of ds_render_scenes; every pointer is a device pointer.  Scene b holds num_objects slots
@@ -393,9 +400,11 @@ DS_API int ds_mesh_catalog_create(int32_t num_models, const int32_t* vertex_offs
                                   const double* raw_half, const double* raw_aabb, const float* kd,
                                   const uint8_t* textures, int32_t texture_size, int32_t device, void** handle);
 DS_API int ds_mesh_catalog_destroy(void* handle);
-/* Sample at pixel centres with a top-left fill rule and no culling; the nearest depth in [near, far] wins, ties go
- * to the lower (slot, face).  DS_ERR_INVALID for a handle that is not a live catalogue or lives on another device,
- * NULL required pointers, batch < 0, num_objects outside [0, 64], an unsupported image size or view volume, and
+/* Sample at pixel centres with a top-left fill rule and no culling; the nearest view depth in [near, far] wins, ties
+ * go to the lower (slot, face).  A perspective face that crosses the near plane draws exactly its part with depth >=
+ * near; depth, world position and UVs are interpolated perspective-correctly.  DS_ERR_INVALID for a handle that is
+ * not a live catalogue or lives on another device, NULL required pointers, batch < 0, num_objects outside [0, 64], an
+ * unsupported image size, projection or view volume (left == right, bottom == top, perspective near <= 0), and
  * (found on the device, so the call waits for `stream`) a model index outside [-1, M), a class index outside the
  * palette, bad floor offsets or a floor texture index outside [-1, num_floor_textures). */
 DS_API int ds_render_scenes(void* handle, const ds_render_camera* camera, const ds_render_args* args, void* stream);

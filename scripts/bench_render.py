@@ -4,6 +4,8 @@
   - render only: ds_render_scenes of B seeded scenes (8 slots, a quarter empty, a floor each) from a synthetic
     catalogue of subdivided boxes, cylinders, wedges and tables (diffuscene_b200.synthetic_meshes, ~20 k faces per
     model at --detail 20): scenes/s and placed triangles/s (the triangles of every non-empty slot and floor);
+  - perspective render only: the same scenes through the completion driver's 512^2 perspective camera
+    (render.REFERENCE_PERSPECTIVE), scenes/s and placed triangles/s;
   - render + device resize + features: the same batch through render.inception_features and render.vgg16_features
     (bf16 extractors, random weights), scenes/s;
   - render -> PNG -> the existing folder path: --png_scenes renders written as PNG, then read back through
@@ -70,6 +72,11 @@ def main(argv=None):
     res["render_ms"] = t * 1e3
     res["render_scenes_per_s"] = a.batch / t
     res["render_triangles_per_s"] = tris / t
+    persp = lambda: R.render_scenes(cat, *args, floors=floors, camera=R.REFERENCE_PERSPECTIVE)
+    t = timed(persp, a.reps)
+    res["perspective_512_render_ms"] = t * 1e3
+    res["perspective_512_scenes_per_s"] = a.batch / t
+    res["perspective_512_triangles_per_s"] = tris / t
 
     inc = F.InceptionFeatures(IR.random_state_dict(seed=5), precision="bf16", capacity=64)
     vgg = I.VGG16Features(he_state_dict(0), precision="bf16", capacity=64)
