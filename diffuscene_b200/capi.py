@@ -89,6 +89,23 @@ DS_RENDER_NO_TEXTURE, DS_RENDER_WHITE_BACKGROUND = 1, 2
 DS_RENDER_ORTHOGRAPHIC, DS_RENDER_PERSPECTIVE = 0, 1
 
 
+class DsSceneBatchArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("num_scenes", "num_class_columns", "objfeat_dim", "layout_h", "layout_w",
+                                         "scaling", "angle_dim", "permute", "num_augmentations")] + \
+        [("augmentations", C.c_int32 * 2), ("batch", C.c_int32), ("num_slots", C.c_int32)] + \
+        [(n, C.c_void_p) for n in ("offsets_dev", "lengths_dev", "class_dev", "translations_dev", "sizes_dev",
+                                   "angles_dev", "objfeats_dev", "layouts_dev")] + \
+        [("bounds_translations", C.c_double * 6), ("bounds_sizes", C.c_double * 6), ("bounds_angles", C.c_double * 2),
+         ("bounds_objfeats", C.c_double * 2)] + \
+        [(n, C.c_void_p) for n in ("scene_index_dev", "rot_angle_dev", "jitter_dev", "perm_key_dev",
+                                   "class_labels_out_dev", "translations_out_dev", "sizes_out_dev", "angles_out_dev",
+                                   "objfeats_out_dev", "length_out_dev", "room_layout_out_dev")]
+
+
+DS_SCENE_AUG_FIXED_ROTATION, DS_SCENE_AUG_ROTATION, DS_SCENE_AUG_JITTER = 1, 2, 3
+DS_SCENE_SCALE, DS_SCENE_SCALE_COSIN_OBJFEATSNORM = 0, 1
+
+
 class DsVlbArgs(C.Structure):
     _fields_ = [
         ("batch", C.c_int32), ("clip_denoised", C.c_int32), ("x0_dev", C.c_void_p), ("seed", C.c_uint64),
@@ -204,6 +221,7 @@ def load(rebuild: bool = False):
         "ds_render_scenes": (C.c_int, [H, C.POINTER(DsRenderCamera), C.POINTER(DsRenderArgs), p]),
         "ds_resize_f32": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p]),
         "ds_resize_u8": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p, p]),
+        "ds_scene_batch": (C.c_int, [C.POINTER(DsSceneBatchArgs), p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
@@ -232,7 +250,8 @@ EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_w
             "ds_inception_create", "ds_inception_destroy", "ds_inception_expected_weight_count",
             "ds_inception_expected_weight", "ds_inception_set_weights", "ds_inception_features",
             "ds_inception_test_conv", "ds_feature_stats", "ds_kid_terms", "ds_mesh_catalog_create",
-            "ds_mesh_catalog_destroy", "ds_render_scenes", "ds_resize_f32", "ds_resize_u8"]
+            "ds_mesh_catalog_destroy", "ds_render_scenes", "ds_resize_f32", "ds_resize_u8",
+            "ds_scene_batch"]
 
 
 class DsError(RuntimeError):

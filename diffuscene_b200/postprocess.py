@@ -52,9 +52,10 @@ def encode_batch(params: Mapping[str, torch.Tensor], bounds: Mapping[str, Sequen
     return out
 
 
-def load_dataset_stats(path: str) -> Dict[str, tuple]:
+def load_dataset_stats(path: str, dtype=None) -> Dict[str, tuple]:
     """`bounds` for encode_batch / post_process_batch from the reference's dataset_stats.txt JSON: bounds_translations
-    / bounds_sizes are 6 floats (lo xyz, hi xyz), bounds_angles 2 (lo, hi), bounds_objfeats[_32] 3 (std, lo, hi)."""
+    / bounds_sizes are 6 floats (lo xyz, hi xyz), bounds_angles 2 (lo, hi), bounds_objfeats[_32] 3 (std, lo, hi).
+    Arrays are float32, or `dtype` (the training data layer keeps the reference's float64)."""
     import json
 
     import numpy as np
@@ -64,7 +65,7 @@ def load_dataset_stats(path: str) -> Dict[str, tuple]:
     for key, n in (("translations", 6), ("sizes", 6), ("angles", 2), ("objfeats", 3), ("objfeats_32", 3)):
         if "bounds_" + key not in stats:
             continue
-        v = np.asarray(stats["bounds_" + key], np.float32).reshape(-1)
+        v = np.asarray(stats["bounds_" + key], np.float32 if dtype is None else dtype).reshape(-1)
         if v.size != n:
             raise ValueError("%s: bounds_%s holds %d values, expected %d" % (path, key, v.size, n))
         out[key] = tuple(np.split(v, n // (3 if n == 6 else 1)))

@@ -137,3 +137,55 @@ class SyntheticShapes(Dataset):
         dense = dense / dense.norm(dim=1).max()
         pick = torch.randint(0, self.N_DENSE, (self.num_points,), generator=g)
         return {"points": dense[pick].float().contiguous(), "label": label, "size": (2 * half).float()}
+
+
+def write_reference_rooms(dataset_directory: str, annotation_file: str, n_rooms: int, max_objects: int = 12,
+                          n_object_classes: int = 21, layout_size: int = 256, seed: int = 0,
+                          splits=("train", "val", "test")) -> list:
+    """Seeded rooms in the reference's preprocessed format, for tests and benchmarks of diffuscene_b200.scene_data:
+    <dataset_directory>/<scene>_<room>/boxes.npz (class_labels one-hot over classes + start + end, translations,
+    sizes, angles, objfeats [L, 64], objfeats_32 [L, 32], a [layout_size, layout_size, 1] uint8 room_layout), the
+    dataset_stats.txt JSON and the splits CSV `annotation_file` (room id, split; room i takes splits[i % len]).
+    Some values fall outside the stats' bounds, so scaling clips them.  Returns the room tags in sorted order."""
+    import os
+    rng = np.random.default_rng(seed)
+    os.makedirs(dataset_directory, exist_ok=True)
+    n_cols = n_object_classes + 2
+    labels = ["class%02d" % c for c in range(n_object_classes)] + ["start", "end"]
+    b = DEFAULT_BOUNDS
+    stats = {"bounds_translations": [float(v) for v in np.concatenate(b["translations"])],
+             "bounds_sizes": [float(v) for v in np.concatenate(b["sizes"])],
+             "bounds_angles": [-3.141592653589793, 3.141592653589793],
+             "bounds_objfeats": [1.25, -5.0, 5.0], "bounds_objfeats_32": [1.0, -4.0, 4.0],
+             "class_labels": labels, "object_types": labels[:-2],
+             "class_frequencies": {k: 1.0 / n_object_classes for k in labels[:-2]},
+             "class_order": {k: i for i, k in enumerate(labels[:-2])}, "count_furniture": {k: 1 for k in labels[:-2]}}
+    with open(os.path.join(dataset_directory, "dataset_stats.txt"), "w") as f:
+        json.dump(stats, f)
+    tags, rows = [], []
+    g = torch.Generator().manual_seed(seed)
+    for i in range(n_rooms):
+        room = "Bedroom-%05d" % i
+        tag = "%08x_%s" % (int(rng.integers(0, 2 ** 31)), room)
+        L = int(rng.integers(1, max_objects + 1))
+        onehot = np.zeros((L, n_cols), np.float32)
+        onehot[np.arange(L), rng.integers(0, n_object_classes, L)] = 1
+        lo_t, hi_t = b["translations"]
+        lo_s, hi_s = b["sizes"]
+        mask = floor_plan_mask(g, layout_size)[0].numpy()
+        os.makedirs(os.path.join(dataset_directory, tag), exist_ok=True)
+        np.savez_compressed(
+            os.path.join(dataset_directory, tag, "boxes.npz"), scene_id=np.array(room), class_labels=onehot,
+            translations=rng.uniform(lo_t * 1.1, hi_t * 1.1, (L, 3)).astype(np.float32),
+            sizes=rng.uniform(lo_s * 0.5, hi_s * 1.05, (L, 3)).astype(np.float32),
+            angles=rng.uniform(-np.pi, np.pi, (L, 1)).astype(np.float32),
+            objfeats=rng.normal(0, 2.0, (L, 64)).astype(np.float32),
+            objfeats_32=rng.normal(0, 1.6, (L, 32)).astype(np.float32),
+            room_layout=(mask[:, :, None] * 255).astype(np.uint8),
+            floor_plan_vertices=np.zeros((0, 3), np.float32), floor_plan_faces=np.zeros((0, 3), np.int32),
+            floor_plan_centroid=np.zeros(3, np.float32))
+        tags.append(tag)
+        rows.append((room, splits[i % len(splits)]))
+    with open(annotation_file, "w") as f:
+        f.write("".join("%s,%s\n" % r for r in rows))
+    return sorted(tags)

@@ -428,6 +428,59 @@ DS_API int ds_resize_u8(const uint8_t* in_dev, int32_t batch, int32_t in_h, int3
                         const int32_t* v_bounds_dev, const int32_t* v_coeffs_dev, int32_t v_ksize,
                         const float* mean_std, float* out_dev, void* stream);
 
+/* ---- training data: batches of preprocessed rooms ----------------------------------------------
+ * ds_scene_batch writes one training batch from a device-resident store of rooms, as the reference's
+ * Diffusion.__getitem__ + default collate give it for a cached_diffusion_* encoding (DESIGN.md, "Training data").
+ * It is a pure function of its inputs: the same arguments give the same bits.
+ *
+ * Store (device): num_scenes rooms whose objects are packed back to back; room s holds lengths[s] objects starting
+ * at offsets[s].  Per object: class [T] int32 (the argmax of the reference's one-hot row over num_class_columns =
+ * object classes + start + end), translations [T, 3], sizes [T, 3], angles [T] fp32, objfeats [T, objfeat_dim] fp32
+ * (objfeat_dim 0: none; else a multiple of 4 and 16-byte aligned).  layouts [num_scenes, layout_h, layout_w] fp32
+ * when layout_h > 0.  Bounds are fp64: translations and sizes (lo xyz, hi xyz), angles (lo, hi), objfeats (lo, hi).
+ *
+ * Per batch row b: scene_index[b]; rot_angle[b] (radians, fp64) for a rotation; jitter[b, 3] (fp64, one draw each
+ * for translations, sizes and angles) for a jitter; perm_key[b, num_slots] fp32 for permute != 0, where object i goes
+ * to the slot of its key's rank among the scene's keys (ties by index).  augmentations[0 .. num_augmentations) apply
+ * in order, at most one rotation and one jitter.  A fixed rotation rotates the layout by round(rot_angle / (pi / 2))
+ * quarter turns (np.rot90); DS_SCENE_AUG_ROTATION with layouts is refused.
+ *
+ * Outputs [batch, num_slots, ...] fp32: class_labels (num_class_columns - 1 columns, +-1, the end label on padding
+ * rows), translations, sizes, angles (angle_dim: 1 under DS_SCENE_SCALE, 2 = (cos, sin) under
+ * DS_SCENE_SCALE_COSIN_OBJFEATSNORM), objfeats (scaled only under the latter), zero on padding rows; length [batch]
+ * int64; room_layout [batch, 1, layout_h, layout_w].  scene_index values outside [0, num_scenes) leave their rows
+ * unwritten and lengths above num_slots are cut to num_slots; callers check both.  DS_ERR_INVALID for NULL required
+ * pointers, batch < 0, num_slots outside [1, 32], an angle_dim the scaling does not write, an unknown or repeated
+ * augmentation, a non-square rotated layout and inconsistent sizes. */
+enum { DS_SCENE_AUG_FIXED_ROTATION = 1, DS_SCENE_AUG_ROTATION = 2, DS_SCENE_AUG_JITTER = 3 };
+enum { DS_SCENE_SCALE = 0, DS_SCENE_SCALE_COSIN_OBJFEATSNORM = 1 };
+typedef struct ds_scene_batch_args {
+  int32_t num_scenes, num_class_columns, objfeat_dim, layout_h, layout_w;
+  int32_t scaling, angle_dim, permute, num_augmentations, augmentations[2];
+  int32_t batch, num_slots;
+  const int32_t* offsets_dev;
+  const int32_t* lengths_dev;
+  const int32_t* class_dev;
+  const float* translations_dev;
+  const float* sizes_dev;
+  const float* angles_dev;
+  const float* objfeats_dev;
+  const float* layouts_dev;
+  double bounds_translations[6], bounds_sizes[6], bounds_angles[2], bounds_objfeats[2];
+  const int64_t* scene_index_dev;
+  const double* rot_angle_dev;
+  const double* jitter_dev;
+  const float* perm_key_dev;
+  float* class_labels_out_dev;
+  float* translations_out_dev;
+  float* sizes_out_dev;
+  float* angles_out_dev;
+  float* objfeats_out_dev;
+  int64_t* length_out_dev;
+  float* room_layout_out_dev;
+} ds_scene_batch_args;
+DS_API int ds_scene_batch(const ds_scene_batch_args* args, void* stream);
+
 /* ---- floor-plan encoder --------------------------------------------------------------------
  * Replaces the ResNet-18 trunk of the reference's room-mask feature extractor (scene_synthesis/networks/
  * feature_extractors.py:19-47 with FrozenBatchNorm2d, frozen_batchnorm.py): conv1 -> bn1 -> ReLU -> maxpool ->

@@ -41,6 +41,7 @@ from training_utils import load_config  # noqa: E402
 
 from diffuscene_b200.collate import collate_scenes  # noqa: E402
 from diffuscene_b200.postprocess import encode_batch, load_dataset_stats, post_process_batch  # noqa: E402
+from diffuscene_b200.scene_data import room_layout  # noqa: E402,F401
 from diffuscene_b200.synthetic import DEFAULT_BOUNDS  # noqa: E402
 
 
@@ -157,14 +158,6 @@ def encode_scenes(scenes, N, bounds, objfeat_dim=0, objectness_dim=0):
     if objfeat_dim > 0:
         parts.append(batch[fkey])
     return torch.cat(parts, dim=-1)
-
-
-def room_layout(s, size):
-    """The reference's room mask (threed_front.py:311-319): room_layout[:, :, 0] resized with PIL bilinear, / 255."""
-    from PIL import Image
-    img = Image.fromarray(np.asarray(s["room_layout"])[:, :, 0])
-    img = img.resize(size, resample=Image.BILINEAR)
-    return np.asarray(img).astype(np.float32) / np.float32(255)
 
 
 def main(argv):

@@ -1,9 +1,14 @@
 #!/usr/bin/env python
 """Training entry point (reference scripts/train_diffusion.py:27-255) on the H100-native network.
 
-Same positional arguments, flags, experiment-directory layout and checkpoint files.  The 3D-FRONT data layer is
-absent in this sandbox, so `--synthetic` (the default) feeds scenes from diffuscene_b200.synthetic with the same
-`sample_params` contract; pass `--no-synthetic` only where scene_synthesis.datasets is importable.
+Same positional arguments, flags, experiment-directory layout and checkpoint files.  `--synthetic` (the default)
+feeds scenes from diffuscene_b200.synthetic with the same `sample_params` contract.  `--no-synthetic` trains on the
+reference's preprocessed 3D-FRONT rooms (<dataset_directory>/<room>/boxes.npz and dataset_stats.txt), held on the
+device by diffuscene_b200.scene_data and batched by one CUDA kernel per batch:
+
+    python scripts/train_diffusion.py CONFIG OUT --no-synthetic --dataset_directory DIR --annotation_file SPLITS.csv
+
+Data settings come from the flags, else from the config's `data` section, else the reference's shipped defaults.
 """
 import argparse
 import os
@@ -19,6 +24,7 @@ from training_utils import id_generator, load_checkpoints, load_config, save_che
 from scene_synthesis.networks import adjust_learning_rate, build_network, optimizer_factory, schedule_factory  # noqa: E402
 from scene_synthesis.stats_logger import StatsLogger  # noqa: E402
 from diffuscene_b200.synthetic import SyntheticScenes, write_stats_file  # noqa: E402
+from diffuscene_b200 import scene_data  # noqa: E402
 
 
 def main(argv):
@@ -27,7 +33,9 @@ def main(argv):
     p.add_argument("output_directory")
     p.add_argument("--weight_file", default=None)
     p.add_argument("--continue_from_epoch", default=0, type=int)
-    p.add_argument("--n_processes", type=int, default=0)
+    p.add_argument("--n_processes", type=int, default=0,
+                   help="DataLoader workers of the synthetic scenes; no effect with --no-synthetic (batches are built "
+                        "on the device)")
     p.add_argument("--seed", type=int, default=27)
     p.add_argument("--experiment_tag", default=None)
     p.add_argument("--with_wandb_logger", action="store_true")
@@ -35,7 +43,33 @@ def main(argv):
     p.add_argument("--synthetic_scenes", type=int, default=2048)
     p.add_argument("--max_epochs", type=int, default=None, help="cap on config training.epochs")
     p.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+    p.add_argument("--dataset_directory", default=None, help="--no-synthetic: the preprocessed rooms (or data."
+                   "dataset_directory)")
+    p.add_argument("--annotation_file", default=None, help="--no-synthetic: the splits CSV (or data.annotation_file)")
+    p.add_argument("--encoding_type", default=None,
+                   help="--no-synthetic: or data.encoding_type, default %s" % scene_data.DEFAULT_ENCODING)
+    p.add_argument("--augmentations", default=None, help="--no-synthetic: comma-separated, or data.augmentations, "
+                   "default %s" % ",".join(scene_data.DEFAULT_AUGMENTATIONS))
+    p.add_argument("--train_stats", default=None,
+                   help="--no-synthetic: stats file in the dataset directory (or data.train_stats, default %s)"
+                        % scene_data.DEFAULT_STATS)
     args = p.parse_args(argv)
+    config = load_config(args.config_file)
+    data = None
+    if not args.synthetic:
+        data = dict(config.get("data") or {})
+        for k in ("dataset_directory", "annotation_file", "encoding_type", "train_stats"):
+            if getattr(args, k) is not None:
+                data[k] = getattr(args, k)
+        if args.augmentations is not None:
+            data["augmentations"] = [a for a in args.augmentations.split(",") if a]
+        for k in ("dataset_directory", "annotation_file"):
+            if not data.get(k):
+                p.error("--no-synthetic needs --%s (or data.%s in the config)" % (k, k))
+        if not os.path.isdir(data["dataset_directory"]):
+            p.error("no dataset directory %s" % data["dataset_directory"])
+        if not os.path.isfile(data["annotation_file"]):
+            p.error("no annotation file %s" % data["annotation_file"])
 
     np.random.seed(args.seed)
     torch.manual_seed(np.random.randint(np.iinfo(np.int32).max))
@@ -49,20 +83,39 @@ def main(argv):
     exp_dir = os.path.join(args.output_directory, tag)
     os.makedirs(exp_dir, exist_ok=True)
     save_experiment_params(args, tag, exp_dir)
-    config = load_config(args.config_file)
 
-    if not args.synthetic:
-        raise RuntimeError("the 3D-FRONT data layer (scene_synthesis.datasets) is outside this repository's scope")
     net_cfg = config["network"]
-    train_ds = SyntheticScenes(net_cfg, args.synthetic_scenes, seed=args.seed)
-    val_ds = SyntheticScenes(net_cfg, max(args.synthetic_scenes // 8, 8), seed=args.seed + 1)
-    np.savez(os.path.join(exp_dir, "bounds.npz"), translations=np.stack(train_ds.bounds["translations"]),
-             sizes=np.stack(train_ds.bounds["sizes"]), angles=np.stack(train_ds.bounds["angles"]))
-    if net_cfg["diffusion_kwargs"].get("loss_iou", False):
-        net_cfg["diffusion_kwargs"]["train_stats_file"] = write_stats_file(os.path.join(exp_dir, "dataset_stats.txt"))
-    train_loader = DataLoader(train_ds, batch_size=config["training"].get("batch_size", 128),
-                              num_workers=args.n_processes, shuffle=True)
-    val_loader = DataLoader(val_ds, batch_size=config["validation"].get("batch_size", 1), num_workers=args.n_processes)
+    if args.synthetic:
+        train_ds = SyntheticScenes(net_cfg, args.synthetic_scenes, seed=args.seed)
+        val_ds = SyntheticScenes(net_cfg, max(args.synthetic_scenes // 8, 8), seed=args.seed + 1)
+        np.savez(os.path.join(exp_dir, "bounds.npz"), translations=np.stack(train_ds.bounds["translations"]),
+                 sizes=np.stack(train_ds.bounds["sizes"]), angles=np.stack(train_ds.bounds["angles"]))
+        if net_cfg["diffusion_kwargs"].get("loss_iou", False):
+            net_cfg["diffusion_kwargs"]["train_stats_file"] = write_stats_file(os.path.join(exp_dir,
+                                                                                            "dataset_stats.txt"))
+        train_loader = DataLoader(train_ds, batch_size=config["training"].get("batch_size", 128),
+                                  num_workers=args.n_processes, shuffle=True)
+        val_loader = DataLoader(val_ds, batch_size=config["validation"].get("batch_size", 1),
+                                num_workers=args.n_processes)
+    else:
+        store_kw = dict(encoding_type=data.get("encoding_type", scene_data.DEFAULT_ENCODING),
+                        train_stats=data.get("train_stats", scene_data.DEFAULT_STATS),
+                        room_layout_size=data.get("room_layout_size", "64,64"), max_length=data.get("max_length"),
+                        device=device)
+        train_ds = scene_data.SceneStore(data["dataset_directory"], data["annotation_file"],
+                                         config["training"].get("splits", ["train", "val"]), net_cfg, **store_kw)
+        val_ds = scene_data.SceneStore(data["dataset_directory"], data["annotation_file"],
+                                       config["validation"].get("splits", ["test"]), net_cfg, **store_kw)
+        b = train_ds.bounds      # the reference's bounds.npz (train_diffusion.py:126-135)
+        np.savez(os.path.join(exp_dir, "bounds.npz"), sizes=b["sizes"], translations=b["translations"],
+                 angles=b["angles"], objfeats=b["objfeats"])
+        net_cfg["diffusion_kwargs"]["train_stats_file"] = train_ds.stats_path
+        train_loader = scene_data.SceneLoader(train_ds, config["training"].get("batch_size", 128), shuffle=True,
+                                              augmentations=data.get("augmentations",
+                                                                     list(scene_data.DEFAULT_AUGMENTATIONS)),
+                                              seed=args.seed)
+        val_loader = scene_data.SceneLoader(val_ds, config["validation"].get("batch_size", 1), shuffle=False,
+                                            augmentations=[], seed=args.seed + 1)
 
     network, train_on_batch, validate_on_batch = build_network(train_ds.feature_size, train_ds.n_classes, config,
                                                                args.weight_file, device=device,
