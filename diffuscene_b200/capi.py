@@ -10,6 +10,8 @@ import ctypes as C
 import os
 from typing import Dict, List, Optional, Tuple
 
+import torch
+
 from . import build as _build
 
 DS_PREC_FP32, DS_PREC_BF16 = 0, 1
@@ -113,6 +115,105 @@ class DsVlbArgs(C.Structure):
         ("reserved", C.c_int32 * 7)]
 
 
+# prototype of every symbol of include/diffuscene_b200.h: name -> (restype, argtypes)
+_H = C.c_void_p
+_p = C.c_void_p
+sig = {
+    "ds_create": (C.c_int, [C.POINTER(DsConfig), C.POINTER(_H)]),
+    "ds_destroy": (C.c_int, [_H]),
+    "ds_last_error": (C.c_char_p, []),
+    "ds_version": (C.c_char_p, []),
+    "ds_load_weight": (C.c_int, [_H, C.c_char_p, _p, C.c_int64]),
+    "ds_commit_weights": (C.c_int, [_H]),
+    "ds_expected_weight_count": (C.c_int, [_H]),
+    "ds_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_set_schedule": (C.c_int, [_H, C.POINTER(DsSchedule)]),
+    "ds_set_vlb_schedule": (C.c_int, [_H, C.c_int32, _p, _p, _p]),
+    "ds_vlb_loop": (C.c_int, [_H, C.POINTER(DsVlbArgs), _p, _p, _p, _p]),
+    "ds_set_context": (C.c_int, [_H, _p, C.c_int32, C.c_int32, _p]),
+    "ds_set_context_cross": (C.c_int, [_H, _p, C.c_int32, C.c_int32, _p]),
+    "ds_denoise_forward": (C.c_int, [_H, _p, _p, _p, C.c_int32, _p]),
+    "ds_denoise_forward_host": (C.c_int, [_H, _p, _p, _p, C.c_int32]),
+    "ds_sample_loop": (C.c_int, [_H, C.POINTER(DsSampleArgs), _p, _p]),
+    "ds_sample_loop_host": (C.c_int, [_H, C.POINTER(DsSampleArgs), _p]),
+    "ds_traj_count": (C.c_int, [C.c_int32, C.c_int32]),
+    "ds_p_sample_step": (C.c_int, [_H, _p, _p, _p, C.c_int32, _p, C.c_int32, _p]),
+    "ds_q_sample": (C.c_int, [_H, _p, _p, _p, _p, C.c_int32, _p]),
+    "ds_p_losses": (C.c_int, [_H, _p, _p, _p, C.c_int32, C.c_int32, _p, _p, _p, C.c_int32, _p]),
+    "ds_train_param_count": (C.c_int64, [_H]),
+    "ds_train_step": (C.c_int, [_H, _p, _p, _p, _p, _p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _p, C.c_float, _p, _p, _p, _p,
+                                C.c_int32, _p]),
+    "ds_train_step_cross": (C.c_int, [_H, _p, _p, _p, _p, _p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _p, C.c_float, _p, _p,
+                                      _p, _p, _p, C.c_int32, _p, C.c_int32, _p]),
+    "ds_train_set_buckets": (C.c_int, [_H, _p, C.c_int32, _p]),
+    "ds_train_phase_ms": (C.c_int, [_H, _p]),
+    "ds_train_read": (C.c_int, [_H, C.c_int32, C.c_int32, _p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _p]),
+    "ds_sumsq": (C.c_int, [_p, C.c_int64, _p, _p]),
+    "ds_adam_step": (C.c_int, [_p, _p, _p, _p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, _p,
+                               C.c_float, _p]),
+    "ds_retrieve_objects": (C.c_int, [_p, C.c_int32, _p, _p, C.c_int32, C.c_int32, _p, _p, _p, C.c_int32, C.c_int32, _p, _p]),
+    "ds_scene_boxes": (C.c_int, [_p, _p, _p, _p, C.c_int32, _p, _p, C.c_int32, _p, _p, C.c_int32, _p, _p]),
+    "ds_scene_stats": (C.c_int, [_p, _p, _p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "ds_plan_describe": (C.c_int, [C.POINTER(DsConfig), C.c_char_p, C.c_int64]),
+    "ds_plan_export_json": (C.c_int, [C.POINTER(DsConfig), C.c_int32, C.c_char_p, C.c_int64]),
+    "ds_enable_taps": (C.c_int, [_H, C.c_int32]),
+    "ds_read_tap": (C.c_int, [_H, C.c_char_p, _p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "ds_launch_count": (C.c_int64, [_H]),
+    "ds_graph_build_count": (C.c_int64, [_H]),
+    "ds_profile_ops": (C.c_int, [_H, C.c_int32, C.c_char_p, C.c_int64, _p, C.c_int32]),
+    "ds_test_gemm_bf16": (C.c_int, [C.c_int, _p, _p, _p, _p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _p]),
+    "ds_room_enc_create": (C.c_int, [C.POINTER(DsRoomEncConfig), C.POINTER(_H)]),
+    "ds_room_enc_destroy": (C.c_int, [_H]),
+    "ds_room_enc_expected_weight_count": (C.c_int, [_H]),
+    "ds_room_enc_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_room_enc_forward": (C.c_int, [_H, _p, _p, C.c_int32, _p, C.c_int32, _p]),
+    "ds_room_enc_backward": (C.c_int, [_H, _p, _p, _p]),
+    "ds_room_enc_read": (C.c_int, [_H, C.c_int32, C.c_int32, _p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _p]),
+    "ds_shape_ae_create": (C.c_int, [C.POINTER(DsShapeAeConfig), C.POINTER(_H)]),
+    "ds_shape_ae_destroy": (C.c_int, [_H]),
+    "ds_shape_ae_expected_weight_count": (C.c_int, [_H]),
+    "ds_shape_ae_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_shape_ae_forward": (C.c_int, [_H, _p, _p, C.c_int32, _p, C.c_int32, C.c_int32, _p, _p, _p, _p]),
+    "ds_shape_ae_train_step": (C.c_int, [_H, _p, _p, C.c_int32, _p, C.c_float, _p, _p, _p]),
+    "ds_shape_ae_set_knn": (C.c_int, [_H, _p]),
+    "ds_shape_ae_get_knn": (C.c_int, [_H, _p, _p]),
+    "ds_knn": (C.c_int, [_p, C.c_int32, C.c_int32, C.c_int32, _p, _p]),
+    "ds_chamfer_forward": (C.c_int, [_p, C.c_int32, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
+    "ds_chamfer_backward": (C.c_int, [_p, C.c_int32, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p, _p, _p]),
+    "ds_text_enc_create": (C.c_int, [C.POINTER(DsTextEncConfig), C.POINTER(_H)]),
+    "ds_text_enc_destroy": (C.c_int, [_H]),
+    "ds_text_enc_expected_weight_count": (C.c_int, [_H]),
+    "ds_text_enc_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_text_enc_set_weights": (C.c_int, [_H, _p, _p]),
+    "ds_text_enc_forward": (C.c_int, [_H, _p, _p, C.c_int32, C.c_int32, _p, _p]),
+    "ds_vgg_create": (C.c_int, [C.POINTER(DsVggConfig), C.POINTER(_H)]),
+    "ds_vgg_destroy": (C.c_int, [_H]),
+    "ds_vgg_expected_weight_count": (C.c_int, [_H]),
+    "ds_vgg_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_vgg_set_weights": (C.c_int, [_H, _p, C.c_int64, _p]),
+    "ds_vgg_features": (C.c_int, [_H, _p, C.c_int32, C.c_int32, C.c_int32, _p, _p]),
+    "ds_vgg_test_conv": (C.c_int, [_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _p, _p, _p, _p]),
+    "ds_manifold_distances": (C.c_int, [_p, C.c_int32, _p, C.c_int32, C.c_int32, _p, _p, _p]),
+    "ds_manifold_radii": (C.c_int, [_p, C.c_int32, C.c_int32, C.c_int32, _p, _p, _p]),
+    "ds_manifold_cover": (C.c_int, [_p, _p, C.c_int32, _p, _p, C.c_int32, C.c_int32, _p, _p, _p, _p, _p]),
+    "ds_inception_create": (C.c_int, [C.POINTER(DsInceptionConfig), C.POINTER(_H)]),
+    "ds_inception_destroy": (C.c_int, [_H]),
+    "ds_inception_expected_weight_count": (C.c_int, [_H]),
+    "ds_inception_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
+    "ds_inception_set_weights": (C.c_int, [_H, _p, C.c_int64, _p]),
+    "ds_inception_features": (C.c_int, [_H, _p, C.c_int32, C.c_int32, C.c_int32, _p, _p]),
+    "ds_inception_test_conv": (C.c_int, [C.c_int32, _p] + [C.c_int32] * 10 + [_p, _p, _p, C.c_int32, C.c_int32, _p]),
+    "ds_feature_stats": (C.c_int, [_p, C.c_int32, C.c_int32, _p, _p, _p]),
+    "ds_kid_terms": (C.c_int, [_p, C.c_int32, _p, C.c_int32, C.c_int32, _p, _p, C.c_int32, C.c_int32, _p, _p]),
+    "ds_mesh_catalog_create": (C.c_int, [C.c_int32, _p, _p, _p, _p, _p, _p, _p, _p, _p, C.c_int32, C.c_int32, C.POINTER(_H)]),
+    "ds_mesh_catalog_destroy": (C.c_int, [_H]),
+    "ds_render_scenes": (C.c_int, [_H, C.POINTER(DsRenderCamera), C.POINTER(DsRenderArgs), _p]),
+    "ds_resize_f32": (C.c_int, [_p] + [C.c_int32] * 5 + [_p, _p, C.c_int32, _p, _p, C.c_int32, _p, _p]),
+    "ds_resize_u8": (C.c_int, [_p] + [C.c_int32] * 5 + [_p, _p, C.c_int32, _p, _p, C.c_int32, _p, _p, _p]),
+    "ds_scene_batch": (C.c_int, [C.POINTER(DsSceneBatchArgs), _p]),
+}
+
+
 _lib = None
 
 
@@ -127,102 +228,6 @@ def load(rebuild: bool = False):
         return _lib
     path = _build.build(force=rebuild)
     lib = C.CDLL(path)
-    H = C.c_void_p
-    p = C.c_void_p
-    sig = {
-        "ds_create": (C.c_int, [C.POINTER(DsConfig), C.POINTER(H)]),
-        "ds_destroy": (C.c_int, [H]),
-        "ds_last_error": (C.c_char_p, []),
-        "ds_version": (C.c_char_p, []),
-        "ds_load_weight": (C.c_int, [H, C.c_char_p, p, C.c_int64]),
-        "ds_commit_weights": (C.c_int, [H]),
-        "ds_expected_weight_count": (C.c_int, [H]),
-        "ds_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_set_schedule": (C.c_int, [H, C.POINTER(DsSchedule)]),
-        "ds_set_vlb_schedule": (C.c_int, [H, C.c_int32, p, p, p]),
-        "ds_vlb_loop": (C.c_int, [H, C.POINTER(DsVlbArgs), p, p, p, p]),
-        "ds_set_context": (C.c_int, [H, p, C.c_int32, C.c_int32, p]),
-        "ds_set_context_cross": (C.c_int, [H, p, C.c_int32, C.c_int32, p]),
-        "ds_denoise_forward": (C.c_int, [H, p, p, p, C.c_int32, p]),
-        "ds_denoise_forward_host": (C.c_int, [H, p, p, p, C.c_int32]),
-        "ds_sample_loop": (C.c_int, [H, C.POINTER(DsSampleArgs), p, p]),
-        "ds_sample_loop_host": (C.c_int, [H, C.POINTER(DsSampleArgs), p]),
-        "ds_traj_count": (C.c_int, [C.c_int32, C.c_int32]),
-        "ds_p_sample_step": (C.c_int, [H, p, p, p, C.c_int32, p, C.c_int32, p]),
-        "ds_q_sample": (C.c_int, [H, p, p, p, p, C.c_int32, p]),
-        "ds_p_losses": (C.c_int, [H, p, p, p, C.c_int32, C.c_int32, p, p, p, C.c_int32, p]),
-        "ds_train_param_count": (C.c_int64, [H]),
-        "ds_train_step": (C.c_int, [H, p, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, C.c_float, p, p, p, p,
-                                    C.c_int32, p]),
-        "ds_train_step_cross": (C.c_int, [H, p, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, C.c_float, p, p,
-                                          p, p, p, C.c_int32, p, C.c_int32, p]),
-        "ds_train_set_buckets": (C.c_int, [H, p, C.c_int32, p]),
-        "ds_train_phase_ms": (C.c_int, [H, p]),
-        "ds_train_read": (C.c_int, [H, C.c_int32, C.c_int32, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), p]),
-        "ds_sumsq": (C.c_int, [p, C.c_int64, p, p]),
-        "ds_adam_step": (C.c_int, [p, p, p, p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int32, p,
-                                   C.c_float, p]),
-        "ds_retrieve_objects": (C.c_int, [p, C.c_int32, p, p, C.c_int32, C.c_int32, p, p, p, C.c_int32, C.c_int32, p, p]),
-        "ds_scene_boxes": (C.c_int, [p, p, p, p, C.c_int32, p, p, C.c_int32, p, p, C.c_int32, p, p]),
-        "ds_scene_stats": (C.c_int, [p, p, p, p, C.c_int32, C.c_int32, p, p, p, p, p, p, p, p]),
-        "ds_plan_describe": (C.c_int, [C.POINTER(DsConfig), C.c_char_p, C.c_int64]),
-        "ds_plan_export_json": (C.c_int, [C.POINTER(DsConfig), C.c_int32, C.c_char_p, C.c_int64]),
-        "ds_enable_taps": (C.c_int, [H, C.c_int32]),
-        "ds_read_tap": (C.c_int, [H, C.c_char_p, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
-        "ds_launch_count": (C.c_int64, [H]),
-        "ds_graph_build_count": (C.c_int64, [H]),
-        "ds_profile_ops": (C.c_int, [H, C.c_int32, C.c_char_p, C.c_int64, p, C.c_int32]),
-        "ds_test_gemm_bf16": (C.c_int, [C.c_int, p, p, p, p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p]),
-        "ds_room_enc_create": (C.c_int, [C.POINTER(DsRoomEncConfig), C.POINTER(H)]),
-        "ds_room_enc_destroy": (C.c_int, [H]),
-        "ds_room_enc_expected_weight_count": (C.c_int, [H]),
-        "ds_room_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_room_enc_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, p]),
-        "ds_room_enc_backward": (C.c_int, [H, p, p, p]),
-        "ds_room_enc_read": (C.c_int, [H, C.c_int32, C.c_int32, p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), p]),
-        "ds_shape_ae_create": (C.c_int, [C.POINTER(DsShapeAeConfig), C.POINTER(H)]),
-        "ds_shape_ae_destroy": (C.c_int, [H]),
-        "ds_shape_ae_expected_weight_count": (C.c_int, [H]),
-        "ds_shape_ae_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_shape_ae_forward": (C.c_int, [H, p, p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p]),
-        "ds_shape_ae_train_step": (C.c_int, [H, p, p, C.c_int32, p, C.c_float, p, p, p]),
-        "ds_shape_ae_set_knn": (C.c_int, [H, p]),
-        "ds_shape_ae_get_knn": (C.c_int, [H, p, p]),
-        "ds_knn": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, p]),
-        "ds_chamfer_forward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p]),
-        "ds_chamfer_backward": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p, p, p, p, p]),
-        "ds_text_enc_create": (C.c_int, [C.POINTER(DsTextEncConfig), C.POINTER(H)]),
-        "ds_text_enc_destroy": (C.c_int, [H]),
-        "ds_text_enc_expected_weight_count": (C.c_int, [H]),
-        "ds_text_enc_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_text_enc_set_weights": (C.c_int, [H, p, p]),
-        "ds_text_enc_forward": (C.c_int, [H, p, p, C.c_int32, C.c_int32, p, p]),
-        "ds_vgg_create": (C.c_int, [C.POINTER(DsVggConfig), C.POINTER(H)]),
-        "ds_vgg_destroy": (C.c_int, [H]),
-        "ds_vgg_expected_weight_count": (C.c_int, [H]),
-        "ds_vgg_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_vgg_set_weights": (C.c_int, [H, p, C.c_int64, p]),
-        "ds_vgg_features": (C.c_int, [H, p, C.c_int32, C.c_int32, C.c_int32, p, p]),
-        "ds_vgg_test_conv": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, p, p, p, p]),
-        "ds_manifold_distances": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, p]),
-        "ds_manifold_radii": (C.c_int, [p, C.c_int32, C.c_int32, C.c_int32, p, p, p]),
-        "ds_manifold_cover": (C.c_int, [p, p, C.c_int32, p, p, C.c_int32, C.c_int32, p, p, p, p, p]),
-        "ds_inception_create": (C.c_int, [C.POINTER(DsInceptionConfig), C.POINTER(H)]),
-        "ds_inception_destroy": (C.c_int, [H]),
-        "ds_inception_expected_weight_count": (C.c_int, [H]),
-        "ds_inception_expected_weight": (C.c_int, [H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
-        "ds_inception_set_weights": (C.c_int, [H, p, C.c_int64, p]),
-        "ds_inception_features": (C.c_int, [H, p, C.c_int32, C.c_int32, C.c_int32, p, p]),
-        "ds_inception_test_conv": (C.c_int, [C.c_int32, p] + [C.c_int32] * 10 + [p, p, p, C.c_int32, C.c_int32, p]),
-        "ds_feature_stats": (C.c_int, [p, C.c_int32, C.c_int32, p, p, p]),
-        "ds_kid_terms": (C.c_int, [p, C.c_int32, p, C.c_int32, C.c_int32, p, p, C.c_int32, C.c_int32, p, p]),
-        "ds_mesh_catalog_create": (C.c_int, [C.c_int32, p, p, p, p, p, p, p, p, p, C.c_int32, C.c_int32, C.POINTER(H)]),
-        "ds_mesh_catalog_destroy": (C.c_int, [H]),
-        "ds_render_scenes": (C.c_int, [H, C.POINTER(DsRenderCamera), C.POINTER(DsRenderArgs), p]),
-        "ds_resize_f32": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p]),
-        "ds_resize_u8": (C.c_int, [p] + [C.c_int32] * 5 + [p, p, C.c_int32, p, p, C.c_int32, p, p, p]),
-        "ds_scene_batch": (C.c_int, [C.POINTER(DsSceneBatchArgs), p]),
-    }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)      # AttributeError here == a symbol of the header is missing
         fn.restype = res
@@ -231,27 +236,7 @@ def load(rebuild: bool = False):
     return lib
 
 
-EXPORTED = ["ds_create", "ds_destroy", "ds_last_error", "ds_version", "ds_load_weight", "ds_commit_weights",
-            "ds_expected_weight_count", "ds_expected_weight", "ds_set_schedule", "ds_set_vlb_schedule", "ds_vlb_loop",
-            "ds_set_context",
-            "ds_set_context_cross", "ds_denoise_forward", "ds_denoise_forward_host", "ds_sample_loop",
-            "ds_sample_loop_host", "ds_traj_count", "ds_p_sample_step", "ds_q_sample", "ds_p_losses", "ds_retrieve_objects",
-            "ds_train_param_count", "ds_train_step", "ds_train_step_cross", "ds_train_set_buckets", "ds_train_phase_ms", "ds_train_read", "ds_sumsq", "ds_adam_step",
-            "ds_plan_describe", "ds_plan_export_json", "ds_enable_taps", "ds_read_tap", "ds_launch_count", "ds_graph_build_count", "ds_profile_ops",
-            "ds_test_gemm_bf16", "ds_room_enc_create", "ds_room_enc_destroy", "ds_room_enc_expected_weight_count",
-            "ds_room_enc_expected_weight", "ds_room_enc_forward", "ds_room_enc_backward", "ds_room_enc_read", "ds_shape_ae_create",
-            "ds_shape_ae_destroy", "ds_shape_ae_expected_weight_count", "ds_shape_ae_expected_weight",
-            "ds_shape_ae_forward", "ds_shape_ae_train_step", "ds_shape_ae_set_knn", "ds_shape_ae_get_knn", "ds_knn",
-            "ds_chamfer_forward", "ds_chamfer_backward", "ds_text_enc_create", "ds_text_enc_destroy",
-            "ds_text_enc_expected_weight_count", "ds_text_enc_expected_weight", "ds_text_enc_set_weights",
-            "ds_text_enc_forward", "ds_scene_boxes", "ds_scene_stats", "ds_vgg_create", "ds_vgg_destroy",
-            "ds_vgg_expected_weight_count", "ds_vgg_expected_weight", "ds_vgg_set_weights", "ds_vgg_features",
-            "ds_vgg_test_conv", "ds_manifold_distances", "ds_manifold_radii", "ds_manifold_cover",
-            "ds_inception_create", "ds_inception_destroy", "ds_inception_expected_weight_count",
-            "ds_inception_expected_weight", "ds_inception_set_weights", "ds_inception_features",
-            "ds_inception_test_conv", "ds_feature_stats", "ds_kid_terms", "ds_mesh_catalog_create",
-            "ds_mesh_catalog_destroy", "ds_render_scenes", "ds_resize_f32", "ds_resize_u8",
-            "ds_scene_batch"]
+EXPORTED = list(sig)
 
 
 class DsError(RuntimeError):
@@ -264,6 +249,120 @@ def check(rc: int):
     if rc < 0:
         raise DsError(rc, load().ds_last_error().decode(errors="replace"))
     return rc
+
+
+def ptr(t: Optional[torch.Tensor]):
+    """The device pointer argument of a tensor (None: NULL)."""
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def stream(device=None):
+    """The stream argument: torch's current stream on `device` (None: the current device)."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def expected_weights(lib, prefix: str, h) -> List[Tuple[str, int]]:
+    """(name, numel) of handle `h`'s flat parameter buffer, in order: <prefix>_expected_weight over
+    <prefix>_expected_weight_count, e.g. prefix "ds_vgg" (the denoiser's is "ds")."""
+    get = getattr(lib, prefix + "_expected_weight")
+    out = []
+    for i in range(check(getattr(lib, prefix + "_expected_weight_count")(h))):
+        name, numel = C.c_char_p(), C.c_int64()
+        check(get(h, i, C.byref(name), C.byref(numel)))
+        out.append((name.value.decode(), numel.value))
+    return out
+
+
+class FeatureNet:
+    """An image feature network on the device: one <prefix>_* handle (create, expected_weight, set_weights, features,
+    destroy) whose weights come from a torchvision-style state dict, uploaded once as one flat fp32 buffer.
+
+    precision "fp32" (default) or "bf16"; `state_dict_or_path` is a state dict, a file holding one, or the module
+    itself.  Calling it with fp32 images [B, 3, H, W] (any device) returns fp32 [B, features] on the device.
+    Subclasses set the symbol prefix, config struct, feature width and the names their messages use."""
+    prefix = ""              # "ds_vgg", "ds_inception"
+    config = None            # DsVggConfig, DsInceptionConfig
+    features = 0
+    name = ""                # the network in messages
+    module = "a module"      # what else a state dict may come from, in the TypeError
+    image_shape = "[B, 3, H, W]"
+    cuda_guard = False       # raise RuntimeError before any library call when torch sees no CUDA device
+
+    def __init__(self, state_dict_or_path, precision: str = "fp32", capacity: Optional[int] = None, device: int = 0):
+        if precision not in ("bf16", "fp32"):
+            raise ValueError("precision must be 'bf16' or 'fp32', not %r" % (precision,))
+        sd = state_dict_or_path
+        if isinstance(sd, (str, os.PathLike)):
+            sd = torch.load(sd, map_location="cpu", weights_only=True)
+        elif isinstance(sd, torch.nn.Module):
+            sd = sd.state_dict()
+        if not isinstance(sd, dict):
+            raise TypeError("%s weights must be a state dict, a state-dict file or %s, not %s"
+                            % (self.name, self.module, type(state_dict_or_path).__name__))
+        if self.cuda_guard and not torch.cuda.is_available():
+            raise RuntimeError("%s needs a CUDA device: diffuscene_b200 has no CPU fallback" % type(self).__name__)
+        self.lib = load()
+        self.device = torch.device("cuda", device)
+        cfg = self.config()
+        cfg.precision = DS_PREC_BF16 if precision == "bf16" else DS_PREC_FP32
+        cfg.capacity = capacity or (64 if precision == "bf16" else 8)
+        cfg.device = device
+        self.capacity = cfg.capacity
+        self.precision = precision
+        self._h = C.c_void_p()
+        check(self._fn("create")(C.byref(cfg), C.byref(self._h)))
+        names = expected_weights(self.lib, self.prefix, self._h)
+        missing = [n for n, _ in names if n not in sd]
+        if missing:
+            self.close()
+            raise KeyError("%s state dict lacks %s" % (self.name, ", ".join(missing)))
+        for n, numel in names:
+            if sd[n].numel() != numel:
+                self.close()
+                raise ValueError("%s has %d elements, expected %d" % (n, sd[n].numel(), numel))
+        flat = torch.cat([sd[n].reshape(-1).float() for n, _ in names]).to(self.device)
+        check(self._fn("set_weights")(self._h, ptr(flat), flat.numel(), stream(self.device)))
+        torch.cuda.current_stream(self.device).synchronize()
+
+    def _fn(self, suffix: str):
+        return getattr(self.lib, self.prefix + "_" + suffix)
+
+    @classmethod
+    def inventory(cls, lib=None, h=None) -> List[Tuple[str, int]]:
+        """(name, numel) of the flat parameter buffer, state-dict order; without `h`, of a temporary fp32 handle of
+        capacity 1 (which needs a device)."""
+        lib = lib or load()
+        if h is not None:
+            return expected_weights(lib, cls.prefix, h)
+        cfg = cls.config()
+        cfg.precision, cfg.capacity = DS_PREC_FP32, 1
+        h = C.c_void_p()
+        check(getattr(lib, cls.prefix + "_create")(C.byref(cfg), C.byref(h)))
+        try:
+            return expected_weights(lib, cls.prefix, h)
+        finally:
+            getattr(lib, cls.prefix + "_destroy")(h)
+
+    def __call__(self, images: torch.Tensor) -> torch.Tensor:
+        if images.dim() != 4 or images.shape[1] != 3:
+            raise ValueError("images must be %s, got %s" % (self.image_shape, tuple(images.shape)))
+        x = images.to(self.device, torch.float32).contiguous()
+        out = torch.empty(x.shape[0], self.features, device=self.device, dtype=torch.float32)
+        if x.shape[0] == 0:
+            return out
+        check(self._fn("features")(self._h, ptr(x), x.shape[0], x.shape[2], x.shape[3], ptr(out), stream(self.device)))
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self._fn("destroy")(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def make_config(spec, num_objects: int, num_timesteps: int, precision: int = DS_PREC_BF16,

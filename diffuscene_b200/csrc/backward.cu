@@ -19,8 +19,6 @@
 
 namespace ds {
 
-static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
-
 // ------------------------------------------------------------------------------------------------
 // GEMMs
 // ------------------------------------------------------------------------------------------------
@@ -176,7 +174,7 @@ __global__ void k_add_block(const T* __restrict__ src, int lds, T* __restrict__ 
 template <typename T>
 void launch_add_block(const T* src, int lds, T* dst, int ldd, int M, int N, int accumulate, cudaStream_t s) {
   const int64_t n = (int64_t)M * N;
-  if (n > 0) k_add_block<T><<<cdiv64(n, 256), 256, 0, s>>>(src, lds, dst, ldd, M, N, accumulate);
+  if (n > 0) k_add_block<T><<<ceil_div(n, 256), 256, 0, s>>>(src, lds, dst, ldd, M, N, accumulate);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -204,7 +202,7 @@ __global__ void k_act(const T* __restrict__ z, int ldz, T* __restrict__ out, int
 template <typename T>
 void launch_act(const T* z, int ldz, T* out, int ldo, int M, int N, int act, cudaStream_t s) {
   const int64_t n = (int64_t)M * N;
-  if (n > 0) k_act<T><<<cdiv64(n, 256), 256, 0, s>>>(z, ldz, out, ldo, M, N, act);
+  if (n > 0) k_act<T><<<ceil_div(n, 256), 256, 0, s>>>(z, ldz, out, ldo, M, N, act);
 }
 // dz = dy * act'(z)
 template <typename T>
@@ -218,7 +216,7 @@ __global__ void k_act_bwd(const T* __restrict__ z, int ldz, const T* __restrict_
 template <typename T>
 void launch_act_bwd(const T* z, int ldz, const T* dy, int ldy, T* dz, int lddz, int M, int N, int act, cudaStream_t s) {
   const int64_t n = (int64_t)M * N;
-  if (n > 0) k_act_bwd<T><<<cdiv64(n, 256), 256, 0, s>>>(z, ldz, dy, ldy, dz, lddz, M, N, act);
+  if (n > 0) k_act_bwd<T><<<ceil_div(n, 256), 256, 0, s>>>(z, ldz, dy, ldy, dz, lddz, M, N, act);
 }
 
 // ---- register-resident variants for the shipped shapes (64 channels per group, N = 12 / 21 objects) -----------------
@@ -380,8 +378,8 @@ bool launch_gn_fwd_reg(const T* in, int ld_in, T* out, int ld_out, const float* 
                        const T* res, int ld_res, int n_scenes, int n_obj, int C, int groups, cudaStream_t s) {
   if (groups != 8 || C != 512 || (n_obj != 12 && n_obj != 21) || n_scenes <= 0) return false;
   const int64_t warps = (int64_t)n_scenes * 8;
-  if (n_obj == 12) k_gn_fwd_reg<T, 12><<<cdiv64(warps, 8), 256, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res, n_scenes, C);
-  else k_gn_fwd_reg<T, 21><<<cdiv64(warps, 8), 256, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res, n_scenes, C);
+  if (n_obj == 12) k_gn_fwd_reg<T, 12><<<ceil_div(warps, 8), 256, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res, n_scenes, C);
+  else k_gn_fwd_reg<T, 21><<<ceil_div(warps, 8), 256, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res, n_scenes, C);
   return true;
 }
 
@@ -486,13 +484,13 @@ void launch_gn_bwd(const T* c, int ldc, const T* dy, int ldy, T* dc, int lddc, T
   if (warps <= 0) return;
   static const int use_reg = getenv("DS_GN_REG") ? atoi(getenv("DS_GN_REG")) : 1;
   if (use_reg && groups == 8 && C == 512 && n_obj == 12)
-    k_gn_bwd_reg<T, 12><<<cdiv64(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
+    k_gn_bwd_reg<T, 12><<<ceil_div(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
                                                          dgamma, dbeta, dfilm, dfilm_row_stride, n_scenes, C);
   else if (use_reg && groups == 8 && C == 512 && n_obj == 21)
-    k_gn_bwd_reg<T, 21><<<cdiv64(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
+    k_gn_bwd_reg<T, 21><<<ceil_div(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
                                                          dgamma, dbeta, dfilm, dfilm_row_stride, n_scenes, C);
   else
-    k_gn_bwd<T><<<cdiv64(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
+    k_gn_bwd<T><<<ceil_div(warps, 8), 256, 0, s>>>(c, ldc, dy, ldy, dc, lddc, dres, ldr, res_accumulate, gamma, beta, film,
                                                  dgamma, dbeta, dfilm, dfilm_row_stride, n_scenes, n_obj, C, groups);
 }
 
@@ -550,7 +548,7 @@ template <typename T>
 void launch_ln_bwd(const T* x, int ldx, const T* dy, int ldy, T* dx, int lddx, int dx_accumulate, T* dres, int ldr,
                    int res_accumulate, const float* g, float* dg, int M, int C, cudaStream_t s) {
   const int rpb = 64;
-  if (M > 0) k_ln_bwd<T><<<cdiv64((int64_t)M, rpb), 256, 0, s>>>(x, ldx, dy, ldy, dx, lddx, dx_accumulate, dres, ldr,
+  if (M > 0) k_ln_bwd<T><<<ceil_div((int64_t)M, rpb), 256, 0, s>>>(x, ldx, dy, ldy, dx, lddx, dx_accumulate, dres, ldr,
                                                                     res_accumulate, g, dg, M, C, rpb);
 }
 
@@ -955,7 +953,7 @@ __global__ void k_pack_piece(const float* __restrict__ src, int rows, int cols, 
 }
 template <typename T>
 void launch_pack_piece(const float* src, int rows, int cols, T* dst, int ldd, int ws, T* dstT, int ldt, cudaStream_t s) {
-  if (rows > 0) k_pack_piece<T><<<cdiv64(rows, 8), 256, 0, s>>>(src, rows, cols, dst, ldd, ws, dstT, ldt);
+  if (rows > 0) k_pack_piece<T><<<ceil_div(rows, 8), 256, 0, s>>>(src, rows, cols, dst, ldd, ws, dstT, ldt);
 }
 // out[c][m] = in[m][c] for m < M, 0 for M <= m < Mcap  (token-major activations -> the K-major operands of dW = dY^T X)
 // colsum (optional): colsum[c] += sum_m in[m][c] -- the bias gradient, for free while the tile is in shared memory
@@ -1026,7 +1024,7 @@ __global__ void k_unpack_piece_grad(const float* __restrict__ dpacked, int ldp, 
 }
 void launch_unpack_piece_grad(const float* dpacked, int ldp, const float* w, int rows, int cols, float* dw, int ws,
                               cudaStream_t s) {
-  if (rows > 0) k_unpack_piece_grad<<<cdiv64(rows, 8), 256, 0, s>>>(dpacked, ldp, w, rows, cols, dw, ws);
+  if (rows > 0) k_unpack_piece_grad<<<ceil_div(rows, 8), 256, 0, s>>>(dpacked, ldp, w, rows, cols, dw, ws);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -8,6 +8,9 @@ namespace ds {
 
 typedef __nv_bfloat16 bf16;
 
+// blocks of `b` threads (or rows) that cover `a`
+__host__ __device__ constexpr int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
 // ---- storage-type traits: activations are float (parity mode) or bf16 (throughput mode) ----
 template <typename T> struct ST;
 template <> struct ST<float> {

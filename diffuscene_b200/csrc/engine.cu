@@ -24,6 +24,29 @@ int fail(int code, const char* fmt, ...) {
   va_end(ap);
   return code;
 }
+static int count_devices(int* ndev) {
+  if (cudaGetDeviceCount(ndev) != cudaSuccess || *ndev == 0) {
+    cudaGetLastError();
+    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  }
+  return 0;
+}
+int require_device() {
+  int ndev = 0;
+  return count_devices(&ndev);
+}
+int open_device(int device) {
+  int ndev = 0;
+  if (const int rc = count_devices(&ndev)) return rc;
+  if (device < 0 || device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", device);
+  CK(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CK(cudaGetDeviceProperties(&prop, device));
+  if (prop.major != 9)
+    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
+                prop.minor);
+  return 0;
+}
 void drop_graph(ds_handle* h) {
   if (h->gexec) cudaGraphExecDestroy(h->gexec);
   h->gexec = nullptr;
@@ -461,18 +484,7 @@ extern "C" const char* ds_version(void) { return "diffuscene_b200 0.1 (sm_90a)";
 extern "C" int ds_create(const ds_config* cfg, ds_handle** out) {
   if (!cfg || !out) return fail(DS_ERR_INVALID, "null argument");
   *out = nullptr;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", cfg->device);
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device,
-                prop.major, prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   ds_handle* h = new ds_handle();
   h->cfg = *cfg;
   if (!build_plan(h->cfg, false, &h->plan)) {
@@ -1129,11 +1141,7 @@ extern "C" int ds_retrieve_objects(const int32_t* class_start_dev, int32_t n_cla
     return fail(DS_ERR_INVALID, "bad argument to ds_retrieve_objects");
   if (mode != 2 && (!cat_feat_dev || !q_feat_dev || feat_dim <= 0)) return fail(DS_ERR_INVALID, "feature arrays needed");
   if (mode != 1 && (!cat_size_dev || !q_size_dev || size_dim <= 0)) return fail(DS_ERR_INVALID, "size arrays needed");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   if (num_queries == 0) return 0;
   launch_retrieve(class_start_dev, n_classes, cat_feat_dev, cat_size_dev, feat_dim, size_dim, q_label_dev, q_feat_dev,
                   q_size_dev, num_queries, mode, out_index_dev, (cudaStream_t)stream);

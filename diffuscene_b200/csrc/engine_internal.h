@@ -28,6 +28,35 @@ int fail(int code, const char* fmt, ...);      // engine.cu: records the message
       return fail(DS_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
   } while (0)
 
+// engine.cu.  require_device(): DS_ERR_NO_DEVICE unless a CUDA device exists.  open_device(): that, then the index is
+// in range, the device is made current and is an sm_90 part.  Both return 0 or the fail() code.
+int require_device();
+int open_device(int device);
+
+// Parameter inventory of a model handle in state-dict order: each tensor's name, size and offset into the flat fp32
+// parameter buffer the handle takes.
+struct WeightTable {
+  std::vector<std::string> names;
+  std::vector<int64_t> numel, off;
+  int64_t total = 0;
+
+  int add(const std::string& name, int64_t n) {
+    names.push_back(name);
+    numel.push_back(n);
+    off.push_back(total);
+    total += n;
+    return int(names.size()) - 1;
+  }
+  int count() const { return int(names.size()); }
+  int get(int index, const char** name, int64_t* n) const {
+    if (!name || !n) return fail(DS_ERR_INVALID, "null argument");
+    if (index < 0 || index >= count()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
+    *name = names[index].c_str();
+    *n = numel[index];
+    return 0;
+  }
+};
+
 // S_POST_LOGVAR .. S_LOG_1MAC are the variational-bound tables of ds_set_vlb_schedule; ds_set_schedule fills the rest
 enum { S_SQRT_AC = 0, S_SQRT_1MAC, S_SQRT_RECIP, S_SQRT_RECIPM1, S_COEF1, S_COEF2, S_SIGMA, S_AC, S_LW, S_NEG_1MAC,
        S_NEG_RECIPM1, S_ZERO, S_ONE, S_POST_LOGVAR, S_MODEL_LOGVAR, S_LOG_1MAC, S_COUNT };

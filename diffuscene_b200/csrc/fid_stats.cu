@@ -198,15 +198,6 @@ __global__ void k_kid_check(const int64_t* __restrict__ idx, int64_t count, int6
   if (i < count && (idx[i] < 0 || idx[i] >= n)) atomicOr(bad, 1);
 }
 
-bool has_device() {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return false;
-  }
-  return true;
-}
-
 }  // namespace
 }  // namespace ds
 
@@ -214,7 +205,7 @@ extern "C" int ds_feature_stats(const float* feats_dev, int32_t n, int32_t d, do
                                 void* stream) {
   if (!feats_dev || !mean_dev || !cov_dev) return fail(DS_ERR_INVALID, "ds_feature_stats: NULL pointer");
   if (n < 2 || d < 1) return fail(DS_ERR_INVALID, "ds_feature_stats: n %d must be >= 2 and d %d >= 1", n, d);
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   k_fs_mean<<<(d + 31) / 32, 256, 0, s>>>(feats_dev, n, d, mean_dev);
   CK(cudaFuncSetAttribute(k_fs_tiles<FS_COV>, cudaFuncAttributeMaxDynamicSharedMemorySize, FS_SMEM));
@@ -236,7 +227,7 @@ extern "C" int ds_kid_terms(const float* real_dev, int32_t n_real, const float* 
     return fail(DS_ERR_INVALID, "ds_kid_terms: m %d must be >= 2 and <= n_real %d, n_fake %d; subsets %d, d %d >= 1", m,
                 n_real, n_fake, subsets, d);
   if ((int64_t)subsets * 3 > 65535) return fail(DS_ERR_INVALID, "ds_kid_terms: %d subsets > 21845", subsets);
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t cnt = (int64_t)subsets * m;
   const int tiles = (m + FS_T - 1) / FS_T;

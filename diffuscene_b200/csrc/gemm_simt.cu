@@ -5,6 +5,8 @@
 // reference's F.conv1d(k=1) / nn.Linear calls (scene_synthesis/networks/denoise_net.py:91,183,214-217).
 // 64x64 output tile per 256-thread CTA, 16-deep k-slices staged transposed in shared memory, 4x4
 // register micro-tile per thread.
+#include <algorithm>
+
 #include "kernels.cuh"
 
 namespace ds {
@@ -89,6 +91,20 @@ void launch_gemm_simt(const GemmArgs& g, bool exact, cudaStream_t s) {
   else k_gemm_simt<T, false><<<grid, 256, 0, s>>>(g);
 }
 void launch_gemm_f32(const GemmArgs& g, cudaStream_t s) { launch_gemm_simt<float>(g, true, s); }
+
+void launch_gemm_simt_chunked(const float* a, int K, const float* w, const float* bias, float* d, int ldd, int M, int N,
+                              int act, cudaStream_t s) {
+  constexpr int CHUNK = 32768 * 64;
+  for (int m0 = 0; m0 < M; m0 += CHUNK) {
+    GemmArgs g = {};
+    g.a0 = a + (size_t)m0 * K; g.lda0 = K; g.k0 = K;
+    g.w = w; g.ldw = K;
+    g.bias = bias;
+    g.d = d + (size_t)m0 * ldd; g.ldd = ldd;
+    g.M = std::min(CHUNK, M - m0); g.N = N; g.act = act;
+    launch_gemm_simt<float>(g, true, s);
+  }
+}
 
 template void launch_gemm_simt<float>(const GemmArgs&, bool, cudaStream_t);
 template void launch_gemm_simt<bf16>(const GemmArgs&, bool, cudaStream_t);

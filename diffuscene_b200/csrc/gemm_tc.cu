@@ -429,6 +429,8 @@ bool tc_runtime_available(char* err, int err_len) {
   return true;
 }
 
+PFN_encodeTiled tc_encode_tiled() { return g_encode; }
+
 static bool encode_2d(CUtensorMap* map, const void* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems,
                       uint32_t box_rows, char* err, int err_len) {
   cuuint64_t dims[2] = {inner, rows};

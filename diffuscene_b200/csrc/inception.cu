@@ -26,8 +26,6 @@ constexpr double IC_BN_EPS = 1e-3;
 enum { T_IN = 0, T_A, T_B, T_T1, T_T2, T_COLS, T_NBUF };
 enum { OP_CONV = 0, OP_MAXPOOL_S2, OP_AVGPOOL_S1, OP_MAXPOOL_S1 };
 
-inline unsigned nblocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // images [B, 3, 299, 299] fp32 in [0, 255] -> x [B, 299, 299, 3] = (v - 128) / 128
 template <typename T>
 __global__ void k_inc_pack(const float* __restrict__ img, T* __restrict__ x, int64_t n) {
@@ -113,16 +111,6 @@ __global__ void k_inc_pool3(const T* __restrict__ in, int C, int H, int W, T* __
   stf(out + i, MAX ? acc : acc / float(cnt));
 }
 
-// fp32 [n] -> bf16 and back (ds_inception_test_conv's output buffer, sentinels included)
-__global__ void k_inc_to_bf16(const float* __restrict__ in, bf16* __restrict__ out, int64_t n) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __float2bfloat16_rn(in[i]);
-}
-__global__ void k_inc_to_f32(const bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __bfloat162float(in[i]);
-}
-
 struct Tens { int slot, H, W, C; };
 
 struct IncConv {
@@ -170,9 +158,7 @@ struct ds_inception {
   ds_inception_config cfg;
   bool bf16 = false;
   size_t esz = 4;
-  std::vector<std::string> names;
-  std::vector<int64_t> numel, off;
-  int64_t n_params = 0;
+  WeightTable w;
   std::vector<IncConv> convs;
   std::vector<IncOp> ops;
   size_t wp_total = 0, b_total = 0;
@@ -192,12 +178,6 @@ void ic_free(ds_inception* h) {
   cudaFree(h->bias);
 }
 
-void add_name(ds_inception* h, const std::string& n, int64_t numel) {
-  h->names.push_back(n);
-  h->numel.push_back(numel);
-  h->off.push_back(h->n_params);
-  h->n_params += numel;
-}
 
 void need(ds_inception* h, const Tens& t) {
   size_t& n = h->buf_n[t.slot];
@@ -216,9 +196,9 @@ struct Net {
     h->wp_total += (size_t)c.cout * c.ld;
     c.b_off = h->b_total;
     h->b_total += c.cout;
-    c.w_idx = int(h->names.size());
-    add_name(h, name + ".conv.weight", (int64_t)cout * c.cin * kh * kw);
-    for (const char* s : {".bn.weight", ".bn.bias", ".bn.running_mean", ".bn.running_var"}) add_name(h, name + s, cout);
+    c.w_idx = int(h->w.names.size());
+    h->w.add(name + ".conv.weight", (int64_t)cout * c.cin * kh * kw);
+    for (const char* s : {".bn.weight", ".bn.bias", ".bn.running_mean", ".bn.running_var"}) h->w.add(name + s, cout);
     if (c.tc_im2col) h->buf_n[T_COLS] = std::max(h->buf_n[T_COLS], (size_t)c.Ho * c.Wo * c.ld);
     const Tens out = {out_slot, c.Ho, c.Wo, pitch ? pitch : cout};
     need(h, out);
@@ -320,20 +300,6 @@ void build_net(ds_inception* h) {
   h->last = x;
 }
 
-void simt(const float* a, int K, const float* w, const float* bias, float* d, int ldd, int M, int N, cudaStream_t s) {
-  constexpr int CHUNK = 32768 * 64;      // gridDim.y of the SIMT GEMM (64 rows per CTA row) stays below 65535
-  for (int m0 = 0; m0 < M; m0 += CHUNK) {
-    GemmArgs g;
-    memset(&g, 0, sizeof g);
-    g.a0 = a + (size_t)m0 * K; g.lda0 = K; g.k0 = K;
-    g.w = w; g.ldw = K;
-    g.bias = bias;
-    g.d = d + (size_t)m0 * ldd; g.ldd = ldd;
-    g.M = std::min(CHUNK, M - m0); g.N = N; g.act = ACT_RELU;
-    launch_gemm_simt<float>(g, true, s);
-  }
-}
-
 // one convolution of B images: in (NHWC, pitch cin) -> out + co_off (pitch ldo)
 template <typename T>
 void conv_fwd(const IncConv& c, const T* in, T* cols, const T* wp, const float* bias, T* out, int ldo, int co_off,
@@ -341,11 +307,11 @@ void conv_fwd(const IncConv& c, const T* in, T* cols, const T* wp, const float* 
   const int64_t M = (int64_t)B * c.Ho * c.Wo;
   if (c.tc_im2col) {
     const int64_t n = M * c.ld;
-    k_inc_im2col<T><<<nblocks(n, 256), 256, 0, s>>>(in, c.cin, c.H, c.W, c.kh, c.kw, c.st, c.ph, c.pw, c.Ho, c.Wo,
+    k_inc_im2col<T><<<ceil_div(n, 256), 256, 0, s>>>(in, c.cin, c.H, c.W, c.kh, c.kw, c.st, c.ph, c.pw, c.Ho, c.Wo,
                                                     c.ld, cols, n);
   }
   if constexpr (std::is_same<T, float>::value) {
-    simt(c.tc_im2col ? cols : in, c.ld, wp, bias, out + co_off, ldo, (int)M, c.cout, s);
+    launch_gemm_simt_chunked(c.tc_im2col ? cols : in, c.ld, wp, bias, out + co_off, ldo, (int)M, c.cout, ACT_RELU, s);
   } else {
     VgConvEpi e;
     memset(&e, 0, sizeof e);
@@ -375,23 +341,15 @@ void run_pass(ds_inception* h, int B, float* feat, cudaStream_t s) {
       conv_fwd<T>(c, in, buf[T_COLS], (const T*)h->wp + c.wp_off, h->bias + c.b_off, out, op.out.C, op.co_off, B, s);
     } else if (op.kind == OP_MAXPOOL_S2) {
       const int64_t n = (int64_t)B * op.out.H * op.out.W * op.in.C;
-      k_inc_maxpool_s2<T><<<nblocks(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, op.out.H, op.out.W, out,
+      k_inc_maxpool_s2<T><<<ceil_div(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, op.out.H, op.out.W, out,
                                                            op.out.C, op.co_off, n);
     } else {
       const int64_t n = (int64_t)B * op.in.H * op.in.W * op.in.C;
-      if (op.kind == OP_MAXPOOL_S1) k_inc_pool3<true, T><<<nblocks(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, out, n);
-      else k_inc_pool3<false, T><<<nblocks(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, out, n);
+      if (op.kind == OP_MAXPOOL_S1) k_inc_pool3<true, T><<<ceil_div(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, out, n);
+      else k_inc_pool3<false, T><<<ceil_div(n, 256), 256, 0, s>>>(in, op.in.C, op.in.H, op.in.W, out, n);
     }
   }
   launch_re_avgpool<T>(buf[h->last.slot], feat, B, h->last.C, h->last.H * h->last.W, s);
-}
-
-bool has_device(int* ndev) {
-  if (cudaGetDeviceCount(ndev) != cudaSuccess || *ndev == 0) {
-    cudaGetLastError();
-    return false;
-  }
-  return true;
 }
 
 }  // namespace
@@ -403,15 +361,7 @@ extern "C" int ds_inception_create(const ds_inception_config* cfg, ds_inception*
     return fail(DS_ERR_INVALID, "inception: precision %d unknown", cfg->precision);
   if (cfg->capacity < 1 || cfg->capacity > 256)
     return fail(DS_ERR_INVALID, "inception: capacity %d outside [1, 256]", cfg->capacity);
-  int ndev = 0;
-  if (!has_device(&ndev)) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", cfg->device);
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
-                prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   if (cfg->precision == DS_PREC_BF16) {
     const int rc = conv_tc_set_attrs();
     if (rc) return rc;
@@ -441,7 +391,7 @@ extern "C" int ds_inception_create(const ds_inception_config* cfg, ds_inception*
                     sizeof err)) {
         ic_free(h);
         delete h;
-        return fail(DS_ERR_CUDA, "inception: tensor maps of %s: %s", h->names[c.w_idx].c_str(), err);
+        return fail(DS_ERR_CUDA, "inception: tensor maps of %s: %s", h->w.names[c.w_idx].c_str(), err);
       }
     }
   }
@@ -459,30 +409,27 @@ extern "C" int ds_inception_destroy(ds_inception* h) {
 
 extern "C" int ds_inception_expected_weight_count(ds_inception* h) {
   if (!h) return fail(DS_ERR_INVALID, "null handle");
-  return int(h->names.size());
+  return h->w.count();
 }
 
 extern "C" int ds_inception_expected_weight(ds_inception* h, int index, const char** name, int64_t* numel) {
-  if (!h || !name || !numel) return fail(DS_ERR_INVALID, "null argument");
-  if (index < 0 || index >= (int)h->names.size()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
-  *name = h->names[index].c_str();
-  *numel = h->numel[index];
-  return 0;
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  return h->w.get(index, name, numel);
 }
 
 extern "C" int ds_inception_set_weights(ds_inception* h, const float* flat_params_dev, int64_t count, void* stream) {
   if (!h || !flat_params_dev) return fail(DS_ERR_INVALID, "null argument");
-  if (count != h->n_params)
+  if (count != h->w.total)
     return fail(DS_ERR_INVALID, "inception: %lld parameters given, %lld expected", (long long)count,
-                (long long)h->n_params);
+                (long long)h->w.total);
   CK(cudaSetDevice(h->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
   float* bn = nullptr;
   CK(cudaMallocAsync((void**)&bn, (size_t)4 * 448 * 4, s));      // [gamma | beta | mean | var] of one convolution
   for (const IncConv& c : h->convs) {
-    const float* w = flat_params_dev + h->off[c.w_idx];
+    const float* w = flat_params_dev + h->w.off[c.w_idx];
     for (int k = 0; k < 4; ++k)
-      CK(cudaMemcpyAsync(bn + k * c.cout, flat_params_dev + h->off[c.w_idx + 1 + k], c.cout * 4,
+      CK(cudaMemcpyAsync(bn + k * c.cout, flat_params_dev + h->w.off[c.w_idx + 1 + k], c.cout * 4,
                          cudaMemcpyDeviceToDevice, s));
     if (h->bf16)
       k_inc_fold<bf16><<<c.cout, 256, 0, s>>>(w, bn, nullptr, c.cin, c.cout, c.kh * c.kw, c.cs, c.ld,
@@ -513,10 +460,10 @@ extern "C" int ds_inception_features(ds_inception* h, const float* images_dev, i
     const int64_t n = (int64_t)B * img_n;
     float* feat = features_dev + (int64_t)b0 * DS_INCEPTION_FEATURES;
     if (h->bf16) {
-      k_inc_pack<bf16><<<nblocks(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, (bf16*)h->buf[T_IN], n);
+      k_inc_pack<bf16><<<ceil_div(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, (bf16*)h->buf[T_IN], n);
       run_pass<bf16>(h, B, feat, s);
     } else {
-      k_inc_pack<float><<<nblocks(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, (float*)h->buf[T_IN], n);
+      k_inc_pack<float><<<ceil_div(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, (float*)h->buf[T_IN], n);
       run_pass<float>(h, B, feat, s);
     }
     CK(cudaGetLastError());
@@ -540,8 +487,7 @@ extern "C" int ds_inception_test_conv(int32_t precision, const float* in_dev, in
   if (out_offset < 0 || out_pitch < out_offset + cout || out_pitch % 8 || out_offset % 8 || cout % 8)
     return fail(DS_ERR_INVALID, "inception conv: output slice [%d, %d) of pitch %d (multiples of 8)", out_offset,
                 out_offset + cout, out_pitch);
-  int ndev = 0;
-  if (!has_device(&ndev)) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   const bool tc = precision == DS_PREC_BF16;
   if (tc) {
     const int rc = conv_tc_set_attrs();
@@ -563,14 +509,14 @@ extern "C" int ds_inception_test_conv(int32_t precision, const float* in_dev, in
     CK(cudaMallocAsync(&x, px * cin * 2, s));
     CK(cudaMallocAsync(&y, n_out * 2, s));
     launch_te_convert<bf16>(in_dev, (bf16*)x, px * cin, s);
-    k_inc_to_bf16<<<nblocks(n_out, 256), 256, 0, s>>>(out_dev, (bf16*)y, n_out);
+    launch_te_convert<bf16>(out_dev, (bf16*)y, n_out, s);      // the output buffer, sentinels included
     k_inc_fold<bf16><<<cout, 256, 0, s>>>(weight_dev, nullptr, bias_dev, cin, cout, kh * kw, c.cs, c.ld, (bf16*)wp, bias);
     char err[256] = "";
     if (conv_maps(c, x, cols, (const bf16*)wp, batch, err, sizeof err)) {
       rc = fail(DS_ERR_CUDA, "inception conv: tensor maps: %s", err);
     } else {
       conv_fwd<bf16>(c, (const bf16*)x, (bf16*)cols, (const bf16*)wp, bias, (bf16*)y, out_pitch, out_offset, batch, s);
-      k_inc_to_f32<<<nblocks(n_out, 256), 256, 0, s>>>((const bf16*)y, out_dev, n_out);
+      launch_widen_bf16((const bf16*)y, out_dev, n_out, s);
     }
     cudaFreeAsync(x, s);
     cudaFreeAsync(y, s);

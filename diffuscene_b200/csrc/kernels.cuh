@@ -1,6 +1,7 @@
 // Host-side launchers of every kernel in the library (definitions in pointwise.cu, gemm_simt.cu,
 // gemm_tc.cu).  All pointers are device pointers; `ld*` are row pitches in elements.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -159,6 +160,7 @@ void launch_te_layernorm(const TI* in, const float* g, const float* b, TO* out, 
 template <typename T>
 void launch_te_attention(const T* qkv, const int* lengths, T* out, int B, int L, int H, cudaStream_t s);
 template <typename T> void launch_te_convert(const float* in, T* out, int64_t n, cudaStream_t s);
+void launch_widen_bf16(const bf16* in, float* out, int64_t n, cudaStream_t s);
 
 // ---- GEMMs: D[M,N] = act([A0 | A1][M, K0+K1] * W[N, K0+K1]^T + bias) (+ residual) -----------------
 struct GemmArgs {
@@ -178,6 +180,10 @@ struct GemmArgs {
   FilmRef film;
 };
 template <typename T> void launch_gemm_simt(const GemmArgs& g, bool exact, cudaStream_t s);
+// fp32 D[M, N] (row pitch ldd) = act(A[M, K] W[N, K]^T + bias) on the exact SIMT GEMM, launched in row chunks that
+// keep gridDim.y (64 rows per CTA row) below 65535
+void launch_gemm_simt_chunked(const float* a, int K, const float* w, const float* bias, float* d, int ldd, int M, int N,
+                              int act, cudaStream_t s);
 // fp32 A/W in, fp32 out (time / context FiLM tables; always fp32)
 void launch_gemm_f32(const GemmArgs& g, cudaStream_t s);
 
@@ -195,6 +201,8 @@ int tc_plan_tiles(const TcGemmPlan* p, int M);
 void tc_plan_set_residual(TcGemmPlan* p, const void* res);      // nullptr: plain store; == output: accumulate in place
 int launch_gemm_tc(const TcGemmPlan* p, int M, cudaStream_t s);   // returns 0 or cudaError
 bool tc_runtime_available(char* err, int err_len);
+// the driver's cuTensorMapEncodeTiled as tc_runtime_available() resolved it (nullptr until that succeeds)
+decltype(&cuTensorMapEncodeTiled) tc_encode_tiled();
 int tc_num_sms();      // SMs of the device tc_runtime_available() checked
 // fused GEMM + channel LayerNorm (+ residual) for K <= 128, N = 512 (gemm_ln.cu): GemmArgs.gamma = LayerNorm gain
 struct LnGemmPlan;

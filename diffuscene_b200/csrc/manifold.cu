@@ -241,15 +241,6 @@ __global__ void k_mf_radii_merge(const double* __restrict__ part, int n, int lis
   radii[i] = lst[k];
 }
 
-bool has_device() {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return false;
-  }
-  return true;
-}
-
 template <int EPI>
 int run_tiles(MfArgs a, int splits, cudaStream_t s) {
   // set on every call: the attribute is per device, and the call may run on any device
@@ -278,7 +269,7 @@ extern "C" int ds_manifold_distances(const double* x_dev, int32_t n, const doubl
   if (!x_dev || !y_dev || !out_dev) return fail(DS_ERR_INVALID, "ds_manifold_distances: NULL x, y or out pointer");
   if (n < 1 || m < 1 || d < 1)
     return fail(DS_ERR_INVALID, "ds_manifold_distances: n %d, m %d and d %d must be >= 1", n, m, d);
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (clamped_dev) CK(cudaMemsetAsync(clamped_dev, 0, 8, s));
   double* nrm = nullptr;
@@ -299,7 +290,7 @@ extern "C" int ds_manifold_radii(const double* x_dev, int32_t n, int32_t d, int3
   if (k < 1 || k > DS_MANIFOLD_MAX_K) return fail(DS_ERR_INVALID, "ds_manifold_radii: k %d outside [1, %d]", k, DS_MANIFOLD_MAX_K);
   if (n <= k) return fail(DS_ERR_INVALID, "ds_manifold_radii: %d features, need more than k = %d", n, k);
   if (d < 1) return fail(DS_ERR_INVALID, "ds_manifold_radii: feature size %d < 1", d);
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (clamped_dev) CK(cudaMemsetAsync(clamped_dev, 0, 8, s));
   int dev = 0, sms = 132;
@@ -343,7 +334,7 @@ extern "C" int ds_manifold_cover(const double* ref_dev, const double* ref_radii_
     return fail(DS_ERR_INVALID, "ds_manifold_cover: reference coverage needs the subject radii");
   if (n_ref < 1 || n_subj < 1 || d < 1)
     return fail(DS_ERR_INVALID, "ds_manifold_cover: n_ref %d, n_subj %d and d %d must be >= 1", n_ref, n_subj, d);
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (clamped_dev) CK(cudaMemsetAsync(clamped_dev, 0, 8, s));
   if (subj_covered_dev) CK(cudaMemsetAsync(subj_covered_dev, 0, n_subj, s));

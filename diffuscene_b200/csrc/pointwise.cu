@@ -51,8 +51,6 @@ static void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
 }
 
 
-static inline int cdiv(int64_t a, int64_t b) { return int((a + b - 1) / b); }
-
 // ------------------------------------------------------------------------------------------------
 // input pack / output unpack
 // ------------------------------------------------------------------------------------------------
@@ -66,7 +64,7 @@ __global__ void k_pack_input(const float* __restrict__ x, T* __restrict__ out, i
 template <typename T>
 void launch_pack_input(const float* x, T* out, int ld_out, int M, int d, cudaStream_t s) {
   int64_t n = (int64_t)M * ld_out;
-  k_pack_input<T><<<cdiv(n, 256), 256, 0, s>>>(x, out, ld_out, M, d);
+  k_pack_input<T><<<ceil_div(n, 256), 256, 0, s>>>(x, out, ld_out, M, d);
 }
 
 template <typename T>
@@ -79,7 +77,7 @@ __global__ void k_unpack_output(const T* __restrict__ in, int ld_in, float* __re
 template <typename T>
 void launch_unpack_output(const T* in, int ld_in, float* out, int M, int d, cudaStream_t s) {
   int64_t n = (int64_t)M * d;
-  k_unpack_output<T><<<cdiv(n, 256), 256, 0, s>>>(in, ld_in, out, M, d);
+  k_unpack_output<T><<<ceil_div(n, 256), 256, 0, s>>>(in, ld_in, out, M, d);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -134,7 +132,7 @@ void launch_groupnorm(const T* in, int ld_in, T* out, int ld_out, const float* g
                       cudaStream_t s) {
   int warps = n_scenes * groups;
   constexpr bool EX = sizeof(T) == 4;
-  k_groupnorm<T, EX><<<cdiv(warps, 4), 128, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res,
+  k_groupnorm<T, EX><<<ceil_div(warps, 4), 128, 0, s>>>(in, ld_in, out, ld_out, gamma, beta, film, res, ld_res,
                                                     n_scenes, n_obj, C, groups);
 }
 
@@ -260,8 +258,8 @@ void launch_layernorm(const T* in, int ld_in, T* out, int ld_out, const float* g
                       int C, cudaStream_t s) {
   constexpr bool EX = sizeof(T) == 4;
   const bool vec_ok = C == 512 && ld_in % 16 == 0 && ld_out % 16 == 0 && (!res || ld_res % 16 == 0);
-  if (vec_ok) launch_pdl(k_layernorm512<T, EX>, dim3(cdiv(M, 8)), dim3(256), 0, s, in, ld_in, out, ld_out, g, res, ld_res, M);
-  else k_layernorm<T, EX><<<cdiv(M, 4), 128, 0, s>>>(in, ld_in, out, ld_out, g, res, ld_res, M, C);
+  if (vec_ok) launch_pdl(k_layernorm512<T, EX>, dim3(ceil_div(M, 8)), dim3(256), 0, s, in, ld_in, out, ld_out, g, res, ld_res, M);
+  else k_layernorm<T, EX><<<ceil_div(M, 4), 128, 0, s>>>(in, ld_in, out, ld_out, g, res, ld_res, M, C);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1026,7 +1024,7 @@ void sinusoid_freqs_host(int dim, float* hf) {
 }
 void launch_sinusoid(float* out, const float* freq_dev, int T, int dim, cudaStream_t s) {
   const int half = dim / 2;
-  k_sinusoid<<<cdiv((int64_t)T * half, 256), 256, 0, s>>>(out, freq_dev, T, dim);
+  k_sinusoid<<<ceil_div((int64_t)T * half, 256), 256, 0, s>>>(out, freq_dev, T, dim);
 }
 // per-sample variant (training: one timestep per scene): out[b][:] = sinusoid(t[b])
 __global__ void k_sinusoid_t(float* __restrict__ out, const float* __restrict__ freq, const int* __restrict__ t, int B,
@@ -1041,7 +1039,7 @@ __global__ void k_sinusoid_t(float* __restrict__ out, const float* __restrict__ 
 }
 void launch_sinusoid_t(float* out, const float* freq_dev, const int* t_dev, int B, int dim, cudaStream_t s) {
   const int half = dim / 2;
-  k_sinusoid_t<<<cdiv((int64_t)B * half, 256), 256, 0, s>>>(out, freq_dev, t_dev, B, dim);
+  k_sinusoid_t<<<ceil_div((int64_t)B * half, 256), 256, 0, s>>>(out, freq_dev, t_dev, B, dim);
 }
 
 __global__ void k_silu_f32(const float* __restrict__ in, float* __restrict__ out, int64_t n) {
@@ -1049,7 +1047,7 @@ __global__ void k_silu_f32(const float* __restrict__ in, float* __restrict__ out
   if (i < n) out[i] = silu_exact(in[i]);
 }
 void launch_silu_f32(const float* in, float* out, int64_t n, cudaStream_t s) {
-  k_silu_f32<<<cdiv(n, 256), 256, 0, s>>>(in, out, n);
+  k_silu_f32<<<ceil_div(n, 256), 256, 0, s>>>(in, out, n);
 }
 
 __global__ void k_t_convert(const int64_t* __restrict__ t, int* __restrict__ out, int B) {
@@ -1057,7 +1055,7 @@ __global__ void k_t_convert(const int64_t* __restrict__ t, int* __restrict__ out
   if (i < B) out[i] = int(t[i]);
 }
 void launch_t_convert(const int64_t* t, int* out, int B, cudaStream_t s) {
-  k_t_convert<<<cdiv(B, 256), 256, 0, s>>>(t, out, B);
+  k_t_convert<<<ceil_div(B, 256), 256, 0, s>>>(t, out, B);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1111,7 +1109,7 @@ void launch_begin_step(const StepCoef* coef, const StepState* st, int* t_dev, fl
     int64_t m = (int64_t)B * ((P * d + 3) / 4);
     if (m > n) n = m;
   }
-  k_begin_step<<<cdiv(n, 256), 256, 0, s>>>(coef, st, t_dev, x, partial, partial_noise, B, n_obj, d, P);
+  k_begin_step<<<ceil_div(n, 256), 256, 0, s>>>(coef, st, t_dev, x, partial, partial_noise, B, n_obj, d, P);
 }
 
 // x0 = a_x*x + a_o*out ; clamp ; x' = c_0*x0 + c_x*x + c_z*z   (rounding order of diffusion_ddpm.py:236-240,
@@ -1171,7 +1169,7 @@ template <typename T>
 void launch_step_update(const StepCoef* coef, StepState* st, float* x, const T* model_out, int ld_out,
                         const float* noise, int B, int n_obj, int d, int clip, cudaStream_t s) {
   int64_t n = (int64_t)B * ((n_obj * d + 3) / 4);
-  k_step_update<T><<<cdiv(n, 256), 256, 0, s>>>(coef, st, x, model_out, ld_out, noise, B, n_obj, d, clip);
+  k_step_update<T><<<ceil_div(n, 256), 256, 0, s>>>(coef, st, x, model_out, ld_out, noise, B, n_obj, d, clip);
 }
 
 __global__ void k_randn(float* __restrict__ out, int B, int per_scene, uint64_t seed, uint64_t scene_offset,
@@ -1191,7 +1189,7 @@ __global__ void k_randn(float* __restrict__ out, int B, int per_scene, uint64_t 
 void launch_randn(float* out, int B, int per_scene, uint64_t seed, uint64_t scene_offset, uint32_t stream_id,
                   cudaStream_t s) {
   int64_t n = (int64_t)B * ((per_scene + 3) / 4);
-  k_randn<<<cdiv(n, 256), 256, 0, s>>>(out, B, per_scene, seed, scene_offset, stream_id);
+  k_randn<<<ceil_div(n, 256), 256, 0, s>>>(out, B, per_scene, seed, scene_offset, stream_id);
 }
 
 template <typename T>
@@ -1218,7 +1216,7 @@ void launch_p_sample(const float* x, const T* model_out, int ld_out, const int* 
                      const float* a_x, const float* a_o, const float* c1, const float* c2, const float* sigma, int B,
                      int n_obj, int d, int clip, cudaStream_t s) {
   int64_t n = (int64_t)B * n_obj * d;
-  k_p_sample<T><<<cdiv(n, 256), 256, 0, s>>>(x, model_out, ld_out, t, noise, out, a_x, a_o, c1, c2, sigma, B, n_obj,
+  k_p_sample<T><<<ceil_div(n, 256), 256, 0, s>>>(x, model_out, ld_out, t, noise, out, a_x, a_o, c1, c2, sigma, B, n_obj,
                                              d, clip);
 }
 
@@ -1234,7 +1232,7 @@ __global__ void k_q_sample(const float* __restrict__ x0, const int64_t* __restri
 void launch_q_sample(const float* x0, const int64_t* t, const float* noise, float* out, const float* sqrt_ac,
                      const float* sqrt_1mac, int B, int per_scene, cudaStream_t s) {
   int64_t n = (int64_t)B * per_scene;
-  k_q_sample<<<cdiv(n, 256), 256, 0, s>>>(x0, t, noise, out, sqrt_ac, sqrt_1mac, B, per_scene);
+  k_q_sample<<<ceil_div(n, 256), 256, 0, s>>>(x0, t, noise, out, sqrt_ac, sqrt_1mac, B, per_scene);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1613,7 +1611,7 @@ void launch_retrieve(const int* class_start, int n_classes, const float* cat_fea
                      int size_dim, const int64_t* q_label, const float* q_feat, const float* q_size, int Q, int mode,
                      int64_t* out, cudaStream_t s) {
   const int wpb = 8;
-  k_retrieve<<<cdiv(Q, wpb), wpb * 32, 0, s>>>(class_start, n_classes, cat_feat, cat_size, feat_dim, size_dim, q_label,
+  k_retrieve<<<ceil_div(Q, wpb), wpb * 32, 0, s>>>(class_start, n_classes, cat_feat, cat_size, feat_dim, size_dim, q_label,
                                                 q_feat, q_size, Q, mode, out);
 }
 

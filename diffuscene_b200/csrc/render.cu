@@ -34,8 +34,6 @@ constexpr float FLOOR_UV_PERIOD = 0.3f;         // floor texture repeats every 3
 enum { RE_MODEL = 1, RE_CLASS = 2, RE_FLOOR_OFF = 4, RE_FLOOR_TEX = 8, RE_FLOOR_COUNT = 16 };
 enum { RF_NO_TEXTURE = 1, RF_WHITE_BACKGROUND = 2 };
 
-inline int cdiv(int64_t a, int64_t b) { return int((a + b - 1) / b); }
-
 struct Catalog {
   int device = 0, M = 0, T = 0;
   int64_t V = 0, F = 0;
@@ -525,15 +523,6 @@ int upload(T** dst, const T* src, int64_t n, const char* what) {
   return 0;
 }
 
-bool has_device() {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return false;
-  }
-  return true;
-}
-
 }  // namespace
 }  // namespace ds
 
@@ -565,7 +554,7 @@ extern "C" int ds_mesh_catalog_create(int32_t num_models, const int32_t* vertex_
       if (!(raw_half[m * 3 + k] > 0.0))
         return fail(DS_ERR_INVALID, "ds_mesh_catalog_create: model %d has a half size <= 0", m);
   }
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   CK(cudaSetDevice(device));
   Catalog* c = new Catalog();
   c->device = device;
@@ -639,7 +628,7 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
       (!a->floor_textures_dev || a->num_floor_textures < 1 || a->floor_texture_size < 1 ||
        a->floor_texture_size > 4096))
     return fail(DS_ERR_INVALID, "ds_render_scenes: floor texture indices need floor textures of size [1, 4096]");
-  if (!has_device()) return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
+  if (const int rc = require_device()) return rc;
   int cur = -1;
   CK(cudaGetDevice(&cur));
   if (cur != c->device)
@@ -702,12 +691,12 @@ extern "C" int ds_render_scenes(void* handle, const ds_render_camera* camera, co
   CK(cudaMallocAsync(&err_dev, sizeof(int), s));
   CK(cudaMemsetAsync(err_dev, 0, sizeof(int), s));
   const bool persp = proj == DS_RENDER_PERSPECTIVE;
-  (persp ? k_render_prep<true> : k_render_prep<false>)<<<cdiv((int64_t)B * (N + 1), 128), 128, 0, s>>>(
+  (persp ? k_render_prep<true> : k_render_prep<false>)<<<ceil_div((int64_t)B * (N + 1), 128), 128, 0, s>>>(
       cam, a->translation_dev, a->size_dev, a->angle_dev, a->model_index_dev, a->class_index_dev, a->num_colors,
       no_tex, c->vert_off, c->verts, c->face_off, c->half, c->aabb, c->M, a->floor_offsets_dev, a->floor_tris_dev,
       a->num_floor_tris, a->floor_texture_index_dev, a->num_floor_textures, B, N, xf, err_dev);
   cudaError_t ce = cudaGetLastError();
-  const int tiles_x = cdiv(cam.W, RT), tiles_y = cdiv(cam.H, RT);
+  const int tiles_x = ceil_div(cam.W, RT), tiles_y = ceil_div(cam.H, RT);
   if (ce == cudaSuccess) {
     (persp ? k_render_tiles<true> : k_render_tiles<false>)<<<dim3(tiles_x * tiles_y, B), RT_THREADS, 0, s>>>(
         cam, xf, a->model_index_dev, a->class_index_dev, a->palette_dev, a->flags, c->vert_off, c->verts, c->face_off,

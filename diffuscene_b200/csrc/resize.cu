@@ -13,8 +13,6 @@ namespace {
 constexpr int PRECISION_BITS = 32 - 8 - 2;      // Pillow's 8-bpc fixed point
 constexpr int MAX_KSIZE = 1024;
 
-inline int cdiv(int64_t a, int64_t b) { return int((a + b - 1) / b); }
-
 __device__ __forceinline__ bool bounds_ok(const int* bd, int o, int ks, int in) {
   const int lo = bd[2 * o], n = bd[2 * o + 1];
   return lo >= 0 && n >= 0 && n <= ks && lo + n <= in;
@@ -109,11 +107,7 @@ int resize(const char* name, const uint8_t* in, int B, int H, int W, int OH, int
     return fail(DS_ERR_INVALID, "%s: sizes %d x %d -> %d x %d outside [1, 4096]", name, H, W, OH, OW);
   if (hks < 1 || hks > MAX_KSIZE || vks < 1 || vks > MAX_KSIZE)
     return fail(DS_ERR_INVALID, "%s: kernel sizes %d, %d outside [1, %d]", name, hks, vks, MAX_KSIZE);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   if (B == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   void* tmp = nullptr;
@@ -121,12 +115,12 @@ int resize(const char* name, const uint8_t* in, int B, int H, int W, int OH, int
   CK(cudaMallocAsync(&tmp, (size_t)B * H * OW * 3 * (F ? sizeof(float) : 1), s));
   CK(cudaMallocAsync(&err_dev, sizeof(int), s));
   CK(cudaMemsetAsync(err_dev, 0, sizeof(int), s));
-  k_resize_h<F><<<cdiv((int64_t)B * H * OW, 256), 256, 0, s>>>(in, B, H, W, OW, hb, hk, hks, tmp, err_dev);
+  k_resize_h<F><<<ceil_div((int64_t)B * H * OW, 256), 256, 0, s>>>(in, B, H, W, OW, hb, hk, hks, tmp, err_dev);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) {
     const float z[6] = {0, 0, 0, 1, 1, 1};
     const float* m = F ? z : ms;
-    k_resize_v<F><<<cdiv((int64_t)B * OH * OW, 256), 256, 0, s>>>(tmp, B, H, OH, OW, vb, vk, vks, m[0], m[1], m[2],
+    k_resize_v<F><<<ceil_div((int64_t)B * OH * OW, 256), 256, 0, s>>>(tmp, B, H, OH, OW, vb, vk, vks, m[0], m[1], m[2],
                                                                   m[3], m[4], m[5], out, err_dev);
     e = cudaGetLastError();
   }

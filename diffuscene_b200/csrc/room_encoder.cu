@@ -23,8 +23,6 @@ template <typename TA, typename TB>
 void launch_gemm_tn(const TA* A, int lda, const TB* B, int ldb, float* D, int ldd, int M, int Ka, int Kb, cudaStream_t s);
 template <typename T> void launch_colsum(const T* A, int lda, float* out, int M, int N, cudaStream_t s);
 
-static inline unsigned re_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // mask [B, C, HW] fp32 (NCHW) -> [B * HW, C] activation rows
 template <typename T>
 __global__ void k_re_pack_mask(const float* __restrict__ m, T* __restrict__ out, int C, int HW, int64_t n) {
@@ -38,7 +36,7 @@ __global__ void k_re_pack_mask(const float* __restrict__ m, T* __restrict__ out,
 template <typename T>
 void launch_re_pack_mask(const float* mask, T* out, int B, int C, int H, int W, cudaStream_t s) {
   const int64_t n = (int64_t)B * H * W * C;
-  if (n > 0) k_re_pack_mask<T><<<re_blocks(n, 256), 256, 0, s>>>(mask, out, C, H * W, n);
+  if (n > 0) k_re_pack_mask<T><<<ceil_div(n, 256), 256, 0, s>>>(mask, out, C, H * W, n);
 }
 
 // cols[r][(ky * k + kx) * Cin + ci] = in[b, oy * stride - pad + ky, ox * stride - pad + kx, ci] (0 outside / in the pad)
@@ -61,7 +59,7 @@ __global__ void k_re_im2col(const T* __restrict__ in, RoomConvGeom g, T* __restr
 template <typename T>
 void launch_re_im2col(const T* in, const RoomConvGeom& g, int B, T* cols, cudaStream_t s) {
   const int64_t n = (int64_t)B * g.hout * g.wout * g.Kp;
-  if (n > 0) k_re_im2col<T><<<re_blocks(n, 256), 256, 0, s>>>(in, g, cols, n);
+  if (n > 0) k_re_im2col<T><<<ceil_div(n, 256), 256, 0, s>>>(in, g, cols, n);
 }
 
 // Adjoint of im2col as a gather: out[b, iy, ix, ci] = sum over the (ky, kx) taps that read it of dcols, in ascending
@@ -98,7 +96,7 @@ template <typename T>
 void launch_re_col2im(const T* dcols, const RoomConvGeom& g, int B, T* out, int accumulate, const T* add, const T* mask,
                       cudaStream_t s) {
   const int64_t n = (int64_t)B * g.hin * g.win * g.cin;
-  if (n > 0) k_re_col2im<T><<<re_blocks(n, 256), 256, 0, s>>>(dcols, g, out, accumulate, add, mask, n);
+  if (n > 0) k_re_col2im<T><<<ceil_div(n, 256), 256, 0, s>>>(dcols, g, out, accumulate, add, mask, n);
 }
 
 // out = relu(z (+ res)); in place allowed (out == z).  NaN passes through, as torch's relu lets it.
@@ -112,7 +110,7 @@ __global__ void k_re_add_relu(const T* z, const T* __restrict__ res, T* out, int
 }
 template <typename T>
 void launch_re_add_relu(const T* z, const T* res, T* out, int64_t n, cudaStream_t s) {
-  if (n > 0) k_re_add_relu<T><<<re_blocks(n, 256), 256, 0, s>>>(z, res, out, n);
+  if (n > 0) k_re_add_relu<T><<<ceil_div(n, 256), 256, 0, s>>>(z, res, out, n);
 }
 
 // 3x3 / stride 2 / pad 1 max pool window of output (oy, ox): torch's argmax, i.e. the first maximum in row-major
@@ -155,7 +153,7 @@ __global__ void k_re_maxpool(const T* __restrict__ in, T* __restrict__ out, int 
 template <typename T>
 void launch_re_maxpool(const T* in, T* out, int B, int C, int hin, int win, int hout, int wout, cudaStream_t s) {
   const int64_t n = (int64_t)B * hout * wout * C;
-  if (n > 0) k_re_maxpool<T><<<re_blocks(n, 256), 256, 0, s>>>(in, out, C, hin, win, hout, wout, n);
+  if (n > 0) k_re_maxpool<T><<<ceil_div(n, 256), 256, 0, s>>>(in, out, C, hin, win, hout, wout, n);
 }
 // max-pool adjoint as a gather: din[b, iy, ix, c] = sum of dout over the windows whose argmax is (iy, ix) (windows in
 // row-major order), zeroed where the pooled input (a ReLU output) is <= 0
@@ -184,7 +182,7 @@ template <typename T>
 void launch_re_maxpool_bwd(const T* in, const T* dout, T* din, int B, int C, int hin, int win, int hout, int wout,
                            cudaStream_t s) {
   const int64_t n = (int64_t)B * hin * win * C;
-  if (n > 0) k_re_maxpool_bwd<T><<<re_blocks(n, 256), 256, 0, s>>>(in, dout, din, C, hin, win, hout, wout, n);
+  if (n > 0) k_re_maxpool_bwd<T><<<ceil_div(n, 256), 256, 0, s>>>(in, dout, din, C, hin, win, hout, wout, n);
 }
 
 // global average pool: feat[b][c] = (sum over the scene's pixels in row-major order) / hw, fp32
@@ -201,7 +199,7 @@ __global__ void k_re_avgpool(const T* __restrict__ in, float* __restrict__ feat,
 template <typename T>
 void launch_re_avgpool(const T* in, float* feat, int B, int C, int hw, cudaStream_t s) {
   const int64_t n = (int64_t)B * C;
-  if (n > 0) k_re_avgpool<T><<<re_blocks(n, 256), 256, 0, s>>>(in, feat, C, hw, n);
+  if (n > 0) k_re_avgpool<T><<<ceil_div(n, 256), 256, 0, s>>>(in, feat, C, hw, n);
 }
 // its adjoint fused with the ReLU adjoint of the last block: d[b, p, c] = (out > 0) * dfeat[b][c] / hw
 template <typename T>
@@ -216,7 +214,7 @@ __global__ void k_re_avgpool_bwd(const float* __restrict__ dfeat, const T* __res
 template <typename T>
 void launch_re_avgpool_bwd(const float* dfeat, const T* out, T* d, int B, int C, int hw, cudaStream_t s) {
   const int64_t n = (int64_t)B * hw * C;
-  if (n > 0) k_re_avgpool_bwd<T><<<re_blocks(n, 256), 256, 0, s>>>(dfeat, out, d, C, hw, n);
+  if (n > 0) k_re_avgpool_bwd<T><<<ceil_div(n, 256), 256, 0, s>>>(dfeat, out, d, C, hw, n);
 }
 
 // FrozenBatchNorm fold, one CTA per output channel: wp[co][(ky, kx, ci)] = W[co][ci][ky][kx] * s (0 in the padding),
@@ -309,9 +307,7 @@ struct ds_room_enc {
   ds_room_enc_config cfg;
   bool bf16 = false;
   size_t esz = 4;
-  std::vector<std::string> names;
-  std::vector<int64_t> numel, off;
-  int64_t n_params = 0;
+  WeightTable w;
   std::vector<RConv> conv;      // stem, then per block: conv1, conv2 (, downsample)
   int blk_first[8];             // index into conv of each block's conv1; downsample follows conv2 when present
   bool blk_ds[8];
@@ -352,12 +348,6 @@ void re_free(ds_room_enc* h) {
   h->kept = false;
 }
 
-void add_name(ds_room_enc* h, const std::string& n, int64_t numel) {
-  h->names.push_back(n);
-  h->numel.push_back(numel);
-  h->off.push_back(h->n_params);
-  h->n_params += numel;
-}
 int add_conv(ds_room_enc* h, const std::string& conv_name, const std::string& bn_name, int cin, int cout, int k, int stride,
              int pad, int hin, int win) {
   RConv c;
@@ -365,10 +355,10 @@ int add_conv(ds_room_enc* h, const std::string& conv_name, const std::string& bn
   c.g.hout = (hin + 2 * pad - k) / stride + 1;
   c.g.wout = (win + 2 * pad - k) / stride + 1;
   c.g.Kp = (k * k * cin + 63) / 64 * 64;
-  c.w_idx = int(h->names.size());
-  add_name(h, conv_name + ".weight", (int64_t)cout * cin * k * k);
-  c.bn_idx = int(h->names.size());
-  for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) add_name(h, bn_name + s, cout);
+  c.w_idx = int(h->w.names.size());
+  h->w.add(conv_name + ".weight", (int64_t)cout * cin * k * k);
+  c.bn_idx = int(h->w.names.size());
+  for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) h->w.add(bn_name + s, cout);
   c.wp_off = h->wp_total;
   h->wp_total += (size_t)cout * c.g.Kp;
   c.b_off = h->b_total;
@@ -459,7 +449,7 @@ int conv_fwd(ds_room_enc* h, int ci, const T* in, T* out, int B, cudaStream_t s)
 template <typename T>
 int re_forward(ds_room_enc* h, const float* prm, const float* mask, int B, float* feat, cudaStream_t s) {
   for (const RConv& c : h->conv)
-    launch_re_fold<T>(prm + h->off[c.w_idx], prm + h->off[c.bn_idx], c.g, P<T>(h->wp, c.wp_off), h->bias + c.b_off, s);
+    launch_re_fold<T>(prm + h->w.off[c.w_idx], prm + h->w.off[c.bn_idx], c.g, P<T>(h->wp, c.wp_off), h->bias + c.b_off, s);
   launch_re_pack_mask<T>(mask, P<T>(h->x0), B, h->cfg.input_channels, h->cfg.height, h->cfg.width, s);
   int rc;
   if ((rc = conv_fwd<T>(h, 0, P<T>(h->x0), P<T>(h->a1), B, s))) return rc;
@@ -505,7 +495,7 @@ template <typename T>
 int re_backward(ds_room_enc* h, const float* dfeat, float* grads, cudaStream_t s) {
   const int B = h->kept_B;
   const float* prm = h->kept_params;
-  CK(cudaMemsetAsync(grads, 0, (size_t)h->n_params * 4, s));
+  CK(cudaMemsetAsync(grads, 0, (size_t)h->w.total * 4, s));
   CK(cudaMemsetAsync(h->dwp, 0, h->dw_total * 4, s));
   CK(cudaMemsetAsync(h->dbias, 0, h->b_total * 4, s));
   {
@@ -533,8 +523,8 @@ int re_backward(ds_room_enc* h, const float* dfeat, float* grads, cudaStream_t s
   launch_re_maxpool_bwd<T>(P<T>(h->a1), P<T>(h->dp), P<T>(h->da1), B, 64, h->H2, h->W2, h->H4, h->W4, s);
   conv_bwd_w<T>(h, 0, P<T>(h->x0), P<T>(h->da1), B, false, s);
   for (const RConv& c : h->conv)
-    launch_re_fold_bwd(h->dwp + c.dw_off, h->dbias + c.b_off, prm + h->off[c.w_idx], prm + h->off[c.bn_idx], c.g,
-                       grads + h->off[c.w_idx], grads + h->off[c.bn_idx], s);
+    launch_re_fold_bwd(h->dwp + c.dw_off, h->dbias + c.b_off, prm + h->w.off[c.w_idx], prm + h->w.off[c.bn_idx], c.g,
+                       grads + h->w.off[c.w_idx], grads + h->w.off[c.bn_idx], s);
   return 0;
 }
 }  // namespace
@@ -549,18 +539,7 @@ extern "C" int ds_room_enc_create(const ds_room_enc_config* cfg, ds_room_enc** o
   if (cfg->height < 32 || cfg->width < 32 || cfg->height % 32 || cfg->width % 32)
     return fail(DS_ERR_INVALID, "room encoder: mask %d x %d must be at least 32 x 32 and a multiple of 32", cfg->height,
                 cfg->width);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", cfg->device);
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
-                prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   if (cfg->precision == DS_PREC_BF16) {
     char err[256] = "";
     if (!tc_runtime_available(err, sizeof err)) return fail(DS_ERR_CUDA, "%s", err);
@@ -611,15 +590,12 @@ extern "C" int ds_room_enc_destroy(ds_room_enc* h) {
 
 extern "C" int ds_room_enc_expected_weight_count(ds_room_enc* h) {
   if (!h) return fail(DS_ERR_INVALID, "null handle");
-  return int(h->names.size());
+  return h->w.count();
 }
 
 extern "C" int ds_room_enc_expected_weight(ds_room_enc* h, int index, const char** name, int64_t* numel) {
-  if (!h || !name || !numel) return fail(DS_ERR_INVALID, "null argument");
-  if (index < 0 || index >= (int)h->names.size()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
-  *name = h->names[index].c_str();
-  *numel = h->numel[index];
-  return 0;
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  return h->w.get(index, name, numel);
 }
 
 extern "C" int ds_room_enc_forward(ds_room_enc* h, const float* flat_params_dev, const float* mask_dev, int32_t batch,
@@ -657,13 +633,6 @@ extern "C" int ds_room_enc_backward(ds_room_enc* h, const float* dfeat_dev, floa
   h->have_grads = true;
   return 0;
 }
-
-namespace {
-__global__ void k_re_widen_bf16(const ds::bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __bfloat162float(in[i]);
-}
-}  // namespace
 
 extern "C" int ds_room_enc_read(ds_room_enc* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity,
                                 int32_t* rows, int32_t* width, void* stream) {
@@ -714,7 +683,7 @@ extern "C" int ds_room_enc_read(ds_room_enc* h, int32_t kind, int32_t index, flo
   CK(cudaSetDevice(h->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
   if (wide) CK(cudaMemcpyAsync(dev_out, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
-  else if (n > 0) k_re_widen_bf16<<<ds::re_blocks(n, 256), 256, 0, s>>>((const ds::bf16*)src, dev_out, n);
+  else launch_widen_bf16((const bf16*)src, dev_out, n, s);
   CK(cudaGetLastError());
   return 0;
 }

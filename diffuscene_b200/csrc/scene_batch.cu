@@ -237,11 +237,7 @@ extern "C" int ds_scene_batch(const ds_scene_batch_args* a, void* stream) {
   if (n_rot && !a->rot_angle_dev) return fail(DS_ERR_INVALID, "ds_scene_batch: a rotation needs rot_angle");
   if (n_jit && !a->jitter_dev) return fail(DS_ERR_INVALID, "ds_scene_batch: a jitter needs jitter draws");
   if (a->permute && !a->perm_key_dev) return fail(DS_ERR_INVALID, "ds_scene_batch: permute needs perm_key");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   if (B == 0) return 0;
   Bounds bd;
   for (int c = 0; c < 3; ++c) {

@@ -16,8 +16,6 @@ constexpr int SE_WARPS = 4;                     // scenes per CTA of k_scene_sta
 
 enum { SE_ERR_OFFSETS = 1, SE_ERR_INDEX = 2 };
 
-inline int cdiv(int64_t a, int64_t b) { return int((a + b - 1) / b); }
-
 __device__ const double k_unit_half[3] = {1, 1, 1}, k_zero_aabb[6] = {0, 0, 0, 0, 0, 0};
 
 // One object: place the model (or the object's own box) and take the bounds of the placed hull.  The placement is
@@ -216,18 +214,14 @@ extern "C" int ds_scene_boxes(const float* translation_dev, const float* size_de
                 num_objects, num_models, num_hull_vertices);
   if (num_models > 0 && (!hull_offsets_dev || !raw_half_dev || !raw_aabb_dev || (num_hull_vertices > 0 && !hull_xz_dev)))
     return fail(DS_ERR_INVALID, "ds_scene_boxes: NULL footprint table for %d models", num_models);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   const int work = std::max(num_objects, num_models);
   if (work == 0) return 0;
   cudaStream_t s = (cudaStream_t)stream;
   int* err_dev = nullptr;
   CK(cudaMallocAsync(&err_dev, sizeof(int), s));
   CK(cudaMemsetAsync(err_dev, 0, sizeof(int), s));
-  k_scene_boxes<<<cdiv(work, 128), 128, 0, s>>>(translation_dev, size_dev, angle_dev, model_index_dev, num_objects,
+  k_scene_boxes<<<ceil_div(work, 128), 128, 0, s>>>(translation_dev, size_dev, angle_dev, model_index_dev, num_objects,
                                                 num_models ? hull_offsets_dev : nullptr, hull_xz_dev,
                                                 num_hull_vertices, raw_half_dev, raw_aabb_dev, num_models, bounds_dev,
                                                 err_dev);
@@ -256,13 +250,9 @@ extern "C" int ds_scene_stats(const double* bounds_dev, const uint8_t* keep_dev,
   if (batch < 0) return fail(DS_ERR_INVALID, "ds_scene_stats: batch %d < 0", batch);
   if (num_objects < 0 || num_objects > SE_MAX_N)
     return fail(DS_ERR_INVALID, "ds_scene_stats: %d objects per scene outside [0, %d]", num_objects, SE_MAX_N);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   if (batch == 0) return 0;
-  k_scene_stats<<<cdiv(batch, SE_WARPS), SE_WARPS * 32, 0, (cudaStream_t)stream>>>(
+  k_scene_stats<<<ceil_div(batch, SE_WARPS), SE_WARPS * 32, 0, (cudaStream_t)stream>>>(
       bounds_dev, keep_dev, class_dev, model_id_dev, batch, num_objects, num_objects_dev, num_pairs_dev, iou_sum_dev,
       insec_count_dev, overlap_ratio_dev, num_symmetry_dev, pair_iou_dev);
   CK(cudaGetLastError());

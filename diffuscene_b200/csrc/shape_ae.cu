@@ -36,8 +36,6 @@ constexpr int GRID_M = GRID_SIDE * GRID_SIDE;      // decoder points per object
 constexpr float BN_EPS = 1e-5f, BN_MOMENTUM = 0.1f;
 constexpr int BN_ROWS = 256;         // rows per partial-statistics chunk
 
-inline unsigned nblk(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // ---- kNN ------------------------------------------------------------------------------------------------------------
 // One thread per query point, QT queries per CTA; candidate tiles of JT points are staged in shared memory.  Distances
 // are sum_c (q_c - x_c)^2 accumulated in channel order with fmaf; CP is C rounded up to 4 (padding channels are 0).
@@ -104,11 +102,11 @@ __global__ void __launch_bounds__(QT) k_sae_knn(const float* __restrict__ x, int
 
 void launch_knn(const float* x, int B, int P, int C, int* idx, cudaStream_t s) {
   if (C <= 4) {
-    k_sae_knn<4, 128, 32><<<dim3(nblk(P, 128), B), 128, 0, s>>>(x, P, C, idx);
+    k_sae_knn<4, 128, 32><<<dim3(ceil_div(P, 128), B), 128, 0, s>>>(x, P, C, idx);
   } else if (C <= 64) {
-    k_sae_knn<64, 64, 16><<<dim3(nblk(P, 64), B), 64, 0, s>>>(x, P, C, idx);
+    k_sae_knn<64, 64, 16><<<dim3(ceil_div(P, 64), B), 64, 0, s>>>(x, P, C, idx);
   } else {
-    k_sae_knn<128, 64, 16><<<dim3(nblk(P, 64), B), 64, 0, s>>>(x, P, C, idx);
+    k_sae_knn<128, 64, 16><<<dim3(ceil_div(P, 64), B), 64, 0, s>>>(x, P, C, idx);
   }
 }
 
@@ -579,9 +577,7 @@ enum { BN_E1, BN_E2, BN_E3, BN_G1, BN_G2, BN_E4, BN_F1A, BN_F1B, BN_F2A, BN_F2B,
 struct ds_shape_ae {
   ds_shape_ae_config cfg;
   int P = 0, F = 0;
-  std::vector<std::string> names;
-  std::vector<int64_t> numel, off;
-  int64_t n_params = 0;
+  WeightTable w;
   SaeLinear conv1, conv2, conv3, gl1, gl2, conv4, mean_fc, logvar_fc, fc, f1[3], f2[3];
   SaeBn bn[BN_COUNT];
   // device buffers (capacity `cap` objects)
@@ -620,26 +616,20 @@ void sae_free(ds_shape_ae* h) {
   h->kept = false;
 }
 
-void add_name(ds_shape_ae* h, const std::string& n, int64_t numel) {
-  h->names.push_back(n);
-  h->numel.push_back(numel);
-  h->off.push_back(h->n_params);
-  h->n_params += numel;
-}
 SaeLinear add_linear(ds_shape_ae* h, const std::string& n, int in, int out) {
   SaeLinear l;
   l.in = in; l.out = out;
-  l.w = h->n_params;
-  add_name(h, n + ".weight", (int64_t)in * out);
-  l.b = h->n_params;
-  add_name(h, n + ".bias", out);
+  l.w = h->w.total;
+  h->w.add(n + ".weight", (int64_t)in * out);
+  l.b = h->w.total;
+  h->w.add(n + ".bias", out);
   return l;
 }
 SaeBn add_bn(ds_shape_ae* h, const std::string& n, int C) {
   SaeBn b;
   b.C = C;
-  b.w = h->n_params;
-  for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) add_name(h, n + s, C);
+  b.w = h->w.total;
+  for (const char* s : {".weight", ".bias", ".running_mean", ".running_var"}) h->w.add(n + s, C);
   return b;
 }
 
@@ -733,15 +723,15 @@ void bn_fwd(ds_shape_ae* h, int i, float* prm, int64_t R, bool train, bool relu,
   float* rv = prm + b.w + 3 * C;
   const int nch = int((R + BN_ROWS - 1) / BN_ROWS);
   if (train) {
-    const dim3 grid(nblk(C, 32), nch), blk(32, 8);
+    const dim3 grid(ceil_div(C, 32), nch), blk(32, 8);
     k_bn_partial<<<grid, blk, 0, s>>>(h->z[i], R, C, nullptr, 0, h->part);
-    k_bn_final<<<nblk(C, 256), 256, 0, s>>>(h->part, nch, C, R, 0, mean, rstd, rm, rv);
+    k_bn_final<<<ceil_div(C, 256), 256, 0, s>>>(h->part, nch, C, R, 0, mean, rstd, rm, rv);
     k_bn_partial<<<grid, blk, 0, s>>>(h->z[i], R, C, mean, 1, h->part);
-    k_bn_final<<<nblk(C, 256), 256, 0, s>>>(h->part, nch, C, R, 1, mean, rstd, rm, rv);
+    k_bn_final<<<ceil_div(C, 256), 256, 0, s>>>(h->part, nch, C, R, 1, mean, rstd, rm, rv);
   } else {
-    k_bn_final<<<nblk(C, 256), 256, 0, s>>>(nullptr, 0, C, R, 2, mean, rstd, rm, rv);
+    k_bn_final<<<ceil_div(C, 256), 256, 0, s>>>(nullptr, 0, C, R, 2, mean, rstd, rm, rv);
   }
-  k_bn_apply<<<nblk(R * C, 256), 256, 0, s>>>(h->z[i], C, mean, rstd, prm + b.w, prm + b.w + C, relu ? 1 : 0, h->y[i],
+  k_bn_apply<<<ceil_div(R * C, 256), 256, 0, s>>>(h->z[i], C, mean, rstd, prm + b.w, prm + b.w + C, relu ? 1 : 0, h->y[i],
                                               R * C);
 }
 // dy (masked by the ReLU when relu) -> dx in place; dgamma / dbeta into grads
@@ -749,24 +739,24 @@ void bn_bwd(ds_shape_ae* h, int i, const float* prm, float* grads, float* d, int
   const SaeBn& b = h->bn[i];
   const int C = b.C;
   const int nch = int((R + BN_ROWS - 1) / BN_ROWS);
-  k_bn_bwd_partial<<<dim3(nblk(C, 32), nch), dim3(32, 8), 0, s>>>(d, h->y[i], h->z[i], bn_mean(h, i), bn_rstd(h, i),
+  k_bn_bwd_partial<<<dim3(ceil_div(C, 32), nch), dim3(32, 8), 0, s>>>(d, h->y[i], h->z[i], bn_mean(h, i), bn_rstd(h, i),
                                                                   R, C, relu ? 1 : 0, h->part);
-  k_bn_bwd_final<<<nblk(C, 256), 256, 0, s>>>(h->part, nch, C, grads + b.w, grads + b.w + C);
-  k_bn_bwd_apply<<<nblk(R * C, 256), 256, 0, s>>>(d, h->y[i], h->z[i], bn_mean(h, i), bn_rstd(h, i), prm + b.w,
+  k_bn_bwd_final<<<ceil_div(C, 256), 256, 0, s>>>(h->part, nch, C, grads + b.w, grads + b.w + C);
+  k_bn_bwd_apply<<<ceil_div(R * C, 256), 256, 0, s>>>(d, h->y[i], h->z[i], bn_mean(h, i), bn_rstd(h, i), prm + b.w,
                                                   grads + b.w, grads + b.w + C, R, C, relu ? 1 : 0, d, R * C);
 }
 
 void nbr_max(ds_shape_ae* h, const float* y, const int* idx, int C, float* out, uint8_t* am, int B, cudaStream_t s) {
   const int64_t n = enc_rows(h, B) * C;
-  k_sae_nbr_max<<<nblk(n, 256), 256, 0, s>>>(y, idx, h->P, C, out, am, n);
+  k_sae_nbr_max<<<ceil_div(n, 256), 256, 0, s>>>(y, idx, h->P, C, out, am, n);
 }
 void build_csr(ds_shape_ae* h, const int* idx, int B, cudaStream_t s) {
   const int64_t R = enc_rows(h, B), n = R * KNN;
   cudaMemsetAsync(h->csr_cnt, 0, (size_t)R * 4, s);
-  k_csr_count<<<nblk(n, 256), 256, 0, s>>>(idx, h->P * KNN, h->P, h->csr_cnt, n);
+  k_csr_count<<<ceil_div(n, 256), 256, 0, s>>>(idx, h->P * KNN, h->P, h->csr_cnt, n);
   k_csr_scan<<<B, 1024, 0, s>>>(h->csr_cnt, h->P, h->P * KNN, B, h->csr_start, h->csr_cur);
-  k_csr_fill<<<nblk(n, 256), 256, 0, s>>>(idx, h->P * KNN, h->P, h->csr_cur, h->csr_list, n);
-  k_csr_sort<<<nblk(R, 128), 128, 0, s>>>(h->csr_start, h->csr_list, R);
+  k_csr_fill<<<ceil_div(n, 256), 256, 0, s>>>(idx, h->P * KNN, h->P, h->csr_cur, h->csr_list, n);
+  k_csr_sort<<<ceil_div(R, 128), 128, 0, s>>>(h->csr_start, h->csr_list, R);
 }
 
 void fold_layer_fwd(ds_shape_ae* h, const SaeLinear* L, int bn0, const float* in, int K, float* cobj, float* out, float* prm,
@@ -774,7 +764,7 @@ void fold_layer_fwd(ds_shape_ae* h, const SaeLinear* L, int bn0, const float* in
   const int64_t Rm = dec_rows(B);
   const int ldw = L[0].in;      // 2 + 512 or 3 + 512
   linear_fwd(h->code_d, 512, prm + L[0].w + K, ldw, prm + L[0].b, cobj, B, 512, s);
-  k_sae_fold_in<<<nblk(Rm * 512, 256), 256, 0, s>>>(in, K, prm + L[0].w, ldw, cobj, GRID_M, 512, h->z[bn0], Rm * 512);
+  k_sae_fold_in<<<ceil_div(Rm * 512, 256), 256, 0, s>>>(in, K, prm + L[0].w, ldw, cobj, GRID_M, 512, h->z[bn0], Rm * 512);
   bn_fwd(h, bn0, prm, Rm, train, true, s);
   linear_fwd(h->y[bn0], 512, prm + L[1].w, 512, prm + L[1].b, h->z[bn0 + 1], Rm, 512, s);
   bn_fwd(h, bn0 + 1, prm, Rm, train, true, s);
@@ -803,13 +793,13 @@ int sae_forward(ds_shape_ae* h, float* prm, const float* points, int B, const fl
   const int P = h->P, F = h->F;
   const int64_t R = enc_rows(h, B), Rm = dec_rows(B);
   CK(cudaMemcpyAsync(h->pts, points, (size_t)R * 3 * 4, cudaMemcpyDeviceToDevice, s));
-  k_sae_grid<<<nblk(Rm, 256), 256, 0, s>>>(h->grid, Rm);
+  k_sae_grid<<<ceil_div(Rm, 256), 256, 0, s>>>(h->grid, Rm);
   if (h->inject)
     for (int i = 0; i < 3; ++i)
       CK(cudaMemcpyAsync(h->knn[i], h->inject + (int64_t)i * R * KNN, (size_t)R * KNN * 4, cudaMemcpyDeviceToDevice, s));
   // encoder (:182-207)
   if (!h->inject) launch_knn(h->pts, B, P, 3, h->knn[0], s);
-  k_sae_cov<<<nblk(R, 128), 128, 0, s>>>(h->pts, h->knn[0], P, h->f12, R);
+  k_sae_cov<<<ceil_div(R, 128), 128, 0, s>>>(h->pts, h->knn[0], P, h->f12, R);
   linear_fwd(h->f12, 12, prm + h->conv1.w, 12, prm + h->conv1.b, h->z[BN_E1], R, 64, s);
   bn_fwd(h, BN_E1, prm, R, train, true, s);
   linear_fwd(h->y[BN_E1], 64, prm + h->conv2.w, 64, prm + h->conv2.b, h->z[BN_E2], R, 64, s);
@@ -830,7 +820,7 @@ int sae_forward(ds_shape_ae* h, float* prm, const float* points, int B, const fl
   // latent head (:349-358) and decoder (:265-282)
   linear_fwd(h->code_e, 512, prm + h->mean_fc.w, 512, prm + h->mean_fc.b, h->mean, B, F, s);
   linear_fwd(h->code_e, 512, prm + h->logvar_fc.w, 512, prm + h->logvar_fc.b, h->lvraw, B, F, s);
-  k_sae_latent<<<nblk(B, 8), 256, 0, s>>>(h->mean, h->lvraw, eps, B, F, h->lat, h->kl);
+  k_sae_latent<<<ceil_div(B, 8), 256, 0, s>>>(h->mean, h->lvraw, eps, B, F, h->lat, h->kl);
   linear_fwd(h->lat, F, prm + h->fc.w, F, prm + h->fc.b, h->code_d, B, 512, s);
   fold_layer_fwd(h, h->f1, BN_F1A, h->grid, 2, h->c1, h->r1, prm, B, train, s);
   fold_layer_fwd(h, h->f2, BN_F2A, h->r1, 3, h->c2, h->rec, prm, B, train, s);
@@ -840,8 +830,8 @@ int sae_forward(ds_shape_ae* h, float* prm, const float* points, int B, const fl
 
 void chamfer_fwd(const float* a, int n, const float* b, int m, int B, float* d1, float* d2, int* i1, int* i2,
                  cudaStream_t s) {
-  k_chamfer_nn<<<dim3(nblk(n, 256), B), 256, 0, s>>>(a, n, b, m, d1, i1);
-  k_chamfer_nn<<<dim3(nblk(m, 256), B), 256, 0, s>>>(b, m, a, n, d2, i2);
+  k_chamfer_nn<<<dim3(ceil_div(n, 256), B), 256, 0, s>>>(a, n, b, m, d1, i1);
+  k_chamfer_nn<<<dim3(ceil_div(m, 256), B), 256, 0, s>>>(b, m, a, n, d2, i2);
 }
 
 // backward of the training loss into grads; the kept forward of the same call provides every activation
@@ -854,15 +844,15 @@ int sae_backward(ds_shape_ae* h, const float* prm, float* grads, int B, float kl
   float* dlat = h->gsmall + (int64_t)B * 512 * 3;
   float* dmean = dlat + (int64_t)B * F;
   float* dlv = dmean + (int64_t)B * F;
-  CK(cudaMemsetAsync(grads, 0, (size_t)h->n_params * 4, s));
+  CK(cudaMemsetAsync(grads, 0, (size_t)h->w.total * 4, s));
   // Chamfer adjoint into the reconstruction, d(dist1) = 1 / (B P), d(dist2) = 1 / (B M)
-  k_chamfer_grad<<<dim3(nblk(GRID_M, 256), B), 256, 0, s>>>(h->rec, GRID_M, h->pts, P, h->cidx2, nullptr,
+  k_chamfer_grad<<<dim3(ceil_div(GRID_M, 256), B), 256, 0, s>>>(h->rec, GRID_M, h->pts, P, h->cidx2, nullptr,
                                                             1.0f / float(Rm), h->cidx1, nullptr, 1.0f / float(R),
                                                             h->drec);
   fold_layer_bwd(h, h->f2, BN_F2A, h->r1, 3, h->drec, h->dr1, dcode, 0, prm, grads, B, s);
   fold_layer_bwd(h, h->f1, BN_F1A, h->grid, 2, h->dr1, nullptr, dcode, 1, prm, grads, B, s);
   linear_bwd(h->lat, dcode, h->fc, prm, grads, dlat, B, s);
-  k_sae_latent_bwd<<<nblk((int64_t)B * F, 256), 256, 0, s>>>(h->mean, h->lvraw, eps, dlat, F, kl_weight / float(B),
+  k_sae_latent_bwd<<<ceil_div((int64_t)B * F, 256), 256, 0, s>>>(h->mean, h->lvraw, eps, dlat, F, kl_weight / float(B),
                                                              dmean, dlv, (int64_t)B * F);
   linear_bwd(h->code_e, dmean, h->mean_fc, prm, grads, dce, B, s);
   launch_gemm_tn<float, float>(dlv, F, h->code_e, 512, grads + h->logvar_fc.w, 512, B, F, 512, s);
@@ -870,17 +860,17 @@ int sae_backward(ds_shape_ae* h, const float* prm, float* grads, int B, float kl
   launch_gemm_nn<float, float, float>(dlv, F, prm + h->logvar_fc.w, 512, dce, 512, B, 512, F, 1, s);
   // encoder, last layer first
   CK(cudaMemsetAsync(h->gA, 0, (size_t)R * 512 * 4, s));
-  k_sae_gmax_bwd<<<nblk(B * 512, 256), 256, 0, s>>>(dce, h->garg, P, 512, h->gA, B * 512);
+  k_sae_gmax_bwd<<<ceil_div(B * 512, 256), 256, 0, s>>>(dce, h->garg, P, 512, h->gA, B * 512);
   bn_bwd(h, BN_E4, prm, grads, h->gA, R, false, s);
   linear_bwd(h->y[BN_G2], h->gA, h->conv4, prm, grads, h->gB, R, s);
   bn_bwd(h, BN_G2, prm, grads, h->gB, R, true, s);
   linear_bwd(h->m2, h->gB, h->gl2, prm, grads, h->gA, R, s);
   build_csr(h, h->knn[2], B, s);
-  k_sae_nbr_max_bwd<<<nblk(R * 128, 256), 256, 0, s>>>(h->gA, h->am2, h->csr_start, h->csr_list, P, 128, h->gB, R * 128);
+  k_sae_nbr_max_bwd<<<ceil_div(R * 128, 256), 256, 0, s>>>(h->gA, h->am2, h->csr_start, h->csr_list, P, 128, h->gB, R * 128);
   bn_bwd(h, BN_G1, prm, grads, h->gB, R, true, s);
   linear_bwd(h->m1, h->gB, h->gl1, prm, grads, h->gA, R, s);
   build_csr(h, h->knn[1], B, s);
-  k_sae_nbr_max_bwd<<<nblk(R * 64, 256), 256, 0, s>>>(h->gA, h->am1, h->csr_start, h->csr_list, P, 64, h->gB, R * 64);
+  k_sae_nbr_max_bwd<<<ceil_div(R * 64, 256), 256, 0, s>>>(h->gA, h->am1, h->csr_start, h->csr_list, P, 64, h->gB, R * 64);
   bn_bwd(h, BN_E3, prm, grads, h->gB, R, true, s);
   linear_bwd(h->y[BN_E2], h->gB, h->conv3, prm, grads, h->gA, R, s);
   bn_bwd(h, BN_E2, prm, grads, h->gA, R, true, s);
@@ -888,16 +878,6 @@ int sae_backward(ds_shape_ae* h, const float* prm, float* grads, int B, float kl
   bn_bwd(h, BN_E1, prm, grads, h->gB, R, true, s);
   linear_bwd(h->f12, h->gB, h->conv1, prm, grads, nullptr, R, s);
   // the running statistics get no gradient: their slots were zeroed above and nothing writes them
-  return 0;
-}
-
-int check_device(int device) {
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
-  if (device < 0 || device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", device);
   return 0;
 }
 }  // namespace
@@ -909,14 +889,7 @@ extern "C" int ds_shape_ae_create(const ds_shape_ae_config* cfg, ds_shape_ae** o
     return fail(DS_ERR_INVALID, "shape auto-encoder: latent_dim %d outside [1, 512]", cfg->latent_dim);
   if (cfg->num_points < KNN)
     return fail(DS_ERR_INVALID, "shape auto-encoder: num_points %d < %d (the kNN size)", cfg->num_points, KNN);
-  int rc = check_device(cfg->device);
-  if (rc) return rc;
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
-                prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   ds_shape_ae* h = new ds_shape_ae();
   h->cfg = *cfg;
   h->P = cfg->num_points;
@@ -962,15 +935,12 @@ extern "C" int ds_shape_ae_destroy(ds_shape_ae* h) {
 
 extern "C" int ds_shape_ae_expected_weight_count(ds_shape_ae* h) {
   if (!h) return fail(DS_ERR_INVALID, "null handle");
-  return int(h->names.size());
+  return h->w.count();
 }
 
 extern "C" int ds_shape_ae_expected_weight(ds_shape_ae* h, int index, const char** name, int64_t* numel) {
-  if (!h || !name || !numel) return fail(DS_ERR_INVALID, "null argument");
-  if (index < 0 || index >= (int)h->names.size()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
-  *name = h->names[index].c_str();
-  *numel = h->numel[index];
-  return 0;
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  return h->w.get(index, name, numel);
 }
 
 extern "C" int ds_shape_ae_forward(ds_shape_ae* h, float* flat_params_dev, const float* points_dev, int32_t batch,
@@ -1063,10 +1033,10 @@ extern "C" int ds_chamfer_backward(const float* a_dev, int32_t n, const float* b
   if (n < 1 || m < 1 || batch < 1) return fail(DS_ERR_INVALID, "chamfer: empty input (n %d, m %d, batch %d)", n, m, batch);
   cudaStream_t s = (cudaStream_t)stream;
   if (grad_a_dev)
-    k_chamfer_grad<<<dim3(nblk(n, 256), batch), 256, 0, s>>>(a_dev, n, b_dev, m, idx1_dev, g1_dev, 0.f, idx2_dev, g2_dev,
+    k_chamfer_grad<<<dim3(ceil_div(n, 256), batch), 256, 0, s>>>(a_dev, n, b_dev, m, idx1_dev, g1_dev, 0.f, idx2_dev, g2_dev,
                                                              0.f, grad_a_dev);
   if (grad_b_dev)
-    k_chamfer_grad<<<dim3(nblk(m, 256), batch), 256, 0, s>>>(b_dev, m, a_dev, n, idx2_dev, g2_dev, 0.f, idx1_dev, g1_dev,
+    k_chamfer_grad<<<dim3(ceil_div(m, 256), batch), 256, 0, s>>>(b_dev, m, a_dev, n, idx2_dev, g2_dev, 0.f, idx1_dev, g1_dev,
                                                              0.f, grad_b_dev);
   CK(cudaGetLastError());
   return 0;

@@ -18,8 +18,6 @@
 
 namespace ds {
 
-static inline unsigned te_blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
 // LayerNorm of one row of H values produced by `val(c)`, one warp per row: mean, then the centred variance (both
 // passes recompute the values, which come from L1), y = (v - mean) / sqrt(var + eps) * g + b.  `valid == false`
 // writes NaN.
@@ -68,12 +66,12 @@ __global__ void __launch_bounds__(256) k_te_layernorm(const TI* __restrict__ in,
 template <typename TO>
 void launch_te_embed_ln(const int* ids, const float* word, const float* pos, const float* type0, const float* g,
                         const float* b, TO* out, int M, int L, int H, int vocab, float eps, cudaStream_t s) {
-  k_te_embed_ln<TO><<<te_blocks(M, 8), 256, 0, s>>>(ids, word, pos, type0, g, b, out, M, L, H, vocab, eps);
+  k_te_embed_ln<TO><<<ceil_div(M, 8), 256, 0, s>>>(ids, word, pos, type0, g, b, out, M, L, H, vocab, eps);
 }
 template <typename TI, typename TO>
 void launch_te_layernorm(const TI* in, const float* g, const float* b, TO* out, int M, int H, float eps,
                          cudaStream_t s) {
-  k_te_layernorm<TI, TO><<<te_blocks(M, 8), 256, 0, s>>>(in, g, b, out, M, H, eps);
+  k_te_layernorm<TI, TO><<<ceil_div(M, 8), 256, 0, s>>>(in, g, b, out, M, H, eps);
 }
 
 // ---- masked self-attention, head dim 64 -------------------------------------------------------------------------
@@ -303,7 +301,14 @@ __global__ void k_te_convert(const float* __restrict__ in, T* __restrict__ out, 
 }
 template <typename T>
 void launch_te_convert(const float* in, T* out, int64_t n, cudaStream_t s) {
-  if (n > 0) k_te_convert<T><<<te_blocks(n, 256), 256, 0, s>>>(in, out, n);
+  if (n > 0) k_te_convert<T><<<ceil_div(n, 256), 256, 0, s>>>(in, out, n);
+}
+__global__ void k_widen_bf16(const bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = __bfloat162float(in[i]);
+}
+void launch_widen_bf16(const bf16* in, float* out, int64_t n, cudaStream_t s) {
+  if (n > 0) k_widen_bf16<<<ceil_div(n, 256), 256, 0, s>>>(in, out, n);
 }
 
 #define INST_TE(T)                                                                                                   \
@@ -332,9 +337,7 @@ struct ds_text_enc {
   ds_text_enc_config cfg;
   bool bf16 = false;
   size_t esz = 4;
-  std::vector<std::string> names;
-  std::vector<int64_t> numel, off;
-  int64_t n_params = 0;
+  WeightTable w;
   bool weights_set = false;
   float* params = nullptr;        // copy of the flat parameters: embeddings, biases and LayerNorm read from here
   void* wmat = nullptr;           // per layer, storage type: [Wq | Wk | Wv] [3H, H], Wo [H, H], W1 [I, H], W2 [H, I]
@@ -356,21 +359,15 @@ void te_release(ds_text_enc* h) {
   delete h;
 }
 
-void add_name(ds_text_enc* h, const std::string& n, int64_t numel) {
-  h->names.push_back(n);
-  h->numel.push_back(numel);
-  h->off.push_back(h->n_params);
-  h->n_params += numel;
-}
 // flat offset of tensor `k` (0 .. 15, state-dict order) of layer `l`
-const float* layer_param(const ds_text_enc* h, const float* base, int l, int k) { return base + h->off[5 + TE_PER_LAYER * l + k]; }
+const float* layer_param(const ds_text_enc* h, const float* base, int l, int k) { return base + h->w.off[5 + TE_PER_LAYER * l + k]; }
 
 template <typename T>
 int te_forward(ds_text_enc* h, const int* ids, const int* lengths, int B, int L, float* out, cudaStream_t s) {
   const ds_text_enc_config& c = h->cfg;
   const int H = c.hidden, M = B * L;
   const float* pr = h->params;
-  launch_te_embed_ln<T>(ids, pr + h->off[0], pr + h->off[1], pr + h->off[2], pr + h->off[3], pr + h->off[4],
+  launch_te_embed_ln<T>(ids, pr + h->w.off[0], pr + h->w.off[1], pr + h->w.off[2], pr + h->w.off[3], pr + h->w.off[4],
                         P<T>(h->x), M, L, H, c.vocab, TE_LN_EPS, s);
   for (int l = 0; l < c.layers; ++l) {
     for (int k = 0; k < 4; ++k) {
@@ -432,18 +429,7 @@ extern "C" int ds_text_enc_create(const ds_text_enc_config* cfg, ds_text_enc** o
                 cfg->max_positions, cfg->type_vocab);
   if (cfg->capacity < 1 || cfg->capacity > TE_MAX_TOKENS)
     return fail(DS_ERR_INVALID, "text encoder: token capacity %d outside [1, %lld]", cfg->capacity, (long long)TE_MAX_TOKENS);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", cfg->device);
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
-                prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   if (cfg->precision == DS_PREC_BF16) {
     char err[256] = "";
     if (!tc_runtime_available(err, sizeof err)) return fail(DS_ERR_CUDA, "%s", err);
@@ -453,35 +439,35 @@ extern "C" int ds_text_enc_create(const ds_text_enc_config* cfg, ds_text_enc** o
   h->bf16 = cfg->precision == DS_PREC_BF16;
   h->esz = h->bf16 ? 2 : 4;
   const int64_t H = cfg->hidden, I = cfg->intermediate;
-  add_name(h, "embeddings.word_embeddings.weight", (int64_t)cfg->vocab * H);
-  add_name(h, "embeddings.position_embeddings.weight", (int64_t)cfg->max_positions * H);
-  add_name(h, "embeddings.token_type_embeddings.weight", (int64_t)cfg->type_vocab * H);
-  add_name(h, "embeddings.LayerNorm.weight", H);
-  add_name(h, "embeddings.LayerNorm.bias", H);
+  h->w.add("embeddings.word_embeddings.weight", (int64_t)cfg->vocab * H);
+  h->w.add("embeddings.position_embeddings.weight", (int64_t)cfg->max_positions * H);
+  h->w.add("embeddings.token_type_embeddings.weight", (int64_t)cfg->type_vocab * H);
+  h->w.add("embeddings.LayerNorm.weight", H);
+  h->w.add("embeddings.LayerNorm.bias", H);
   size_t wtotal = 0;
   for (int l = 0; l < cfg->layers; ++l) {
     const std::string pre = "encoder.layer." + std::to_string(l) + ".";
     for (const char* n : {"query", "key", "value"}) {
-      add_name(h, pre + "attention.self." + n + ".weight", H * H);
-      add_name(h, pre + "attention.self." + n + ".bias", H);
+      h->w.add(pre + "attention.self." + n + ".weight", H * H);
+      h->w.add(pre + "attention.self." + n + ".bias", H);
     }
-    add_name(h, pre + "attention.output.dense.weight", H * H);
-    add_name(h, pre + "attention.output.dense.bias", H);
-    add_name(h, pre + "attention.output.LayerNorm.weight", H);
-    add_name(h, pre + "attention.output.LayerNorm.bias", H);
-    add_name(h, pre + "intermediate.dense.weight", I * H);
-    add_name(h, pre + "intermediate.dense.bias", I);
-    add_name(h, pre + "output.dense.weight", H * I);
-    add_name(h, pre + "output.dense.bias", H);
-    add_name(h, pre + "output.LayerNorm.weight", H);
-    add_name(h, pre + "output.LayerNorm.bias", H);
+    h->w.add(pre + "attention.output.dense.weight", H * H);
+    h->w.add(pre + "attention.output.dense.bias", H);
+    h->w.add(pre + "attention.output.LayerNorm.weight", H);
+    h->w.add(pre + "attention.output.LayerNorm.bias", H);
+    h->w.add(pre + "intermediate.dense.weight", I * H);
+    h->w.add(pre + "intermediate.dense.bias", I);
+    h->w.add(pre + "output.dense.weight", H * I);
+    h->w.add(pre + "output.dense.bias", H);
+    h->w.add(pre + "output.LayerNorm.weight", H);
+    h->w.add(pre + "output.LayerNorm.bias", H);
     for (int64_t n : {3 * H * H, H * H, I * H, H * I}) {
       h->w_off.push_back(wtotal);
       wtotal += (size_t)n;
     }
   }
   const size_t cap = (size_t)cfg->capacity, e = h->esz;
-  cudaError_t err = cudaMalloc(&h->params, (size_t)h->n_params * 4);
+  cudaError_t err = cudaMalloc(&h->params, (size_t)h->w.total * 4);
   if (err == cudaSuccess) err = cudaMalloc(&h->wmat, wtotal * e);
   if (err == cudaSuccess) err = cudaMalloc(&h->bqkv, (size_t)cfg->layers * 3 * H * 4);
   if (err == cudaSuccess) err = cudaMalloc(&h->x, cap * H * e);
@@ -537,22 +523,19 @@ extern "C" int ds_text_enc_destroy(ds_text_enc* h) {
 
 extern "C" int ds_text_enc_expected_weight_count(ds_text_enc* h) {
   if (!h) return fail(DS_ERR_INVALID, "null handle");
-  return int(h->names.size());
+  return h->w.count();
 }
 
 extern "C" int ds_text_enc_expected_weight(ds_text_enc* h, int index, const char** name, int64_t* numel) {
-  if (!h || !name || !numel) return fail(DS_ERR_INVALID, "null argument");
-  if (index < 0 || index >= (int)h->names.size()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
-  *name = h->names[index].c_str();
-  *numel = h->numel[index];
-  return 0;
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  return h->w.get(index, name, numel);
 }
 
 extern "C" int ds_text_enc_set_weights(ds_text_enc* h, const float* flat_params_dev, void* stream) {
   if (!h || !flat_params_dev) return fail(DS_ERR_INVALID, "null argument");
   CK(cudaSetDevice(h->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaMemcpyAsync(h->params, flat_params_dev, (size_t)h->n_params * 4, cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(h->params, flat_params_dev, (size_t)h->w.total * 4, cudaMemcpyDeviceToDevice, s));
   if (h->bf16) te_pack<bf16>(h, s);
   else te_pack<float>(h, s);
   CK(cudaGetLastError());

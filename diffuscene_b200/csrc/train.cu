@@ -955,13 +955,6 @@ extern "C" int ds_train_phase_ms(ds_handle* h, float* out6) {
   return 0;
 }
 
-namespace {
-__global__ void k_widen_bf16(const ds::bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __bfloat162float(in[i]);
-}
-}  // namespace
-
 extern "C" int ds_train_read(ds_handle* h, int32_t kind, int32_t index, float* dev_out, int64_t capacity, int32_t* rows,
                              int32_t* width, void* stream) {
   if (!h) return fail(DS_ERR_INVALID, "null argument");
@@ -1027,7 +1020,7 @@ extern "C" int ds_train_read(ds_handle* h, int32_t kind, int32_t index, float* d
   CK(cudaSetDevice(h->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
   if (wide) CK(cudaMemcpyAsync(dev_out, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
-  else if (n > 0) k_widen_bf16<<<(n + 255) / 256, 256, 0, s>>>((const ds::bf16*)src, dev_out, n);
+  else launch_widen_bf16((const bf16*)src, dev_out, n, s);
   CK(cudaGetLastError());
   return 0;
 }

@@ -255,28 +255,6 @@ __global__ void k_vgg_fill_bias(const float* __restrict__ bias, float* __restric
   if (i < n) out[i] = bias[i % N];
 }
 
-__global__ void k_vgg_bf16_to_f32(const bf16* __restrict__ in, float* __restrict__ out, int64_t n) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __bfloat162float(in[i]);
-}
-
-inline unsigned blocks(int64_t n, int t) { return (unsigned)((n + t - 1) / t); }
-
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled vg_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (PFN_encodeTiled)p;
-  }
-  return fn;
-}
-
 struct VgConv {
   RoomConvGeom g;         // stride 1, pad 1 (the first layer: its 3 x 3 x 3 im2col as a 1 x 1 convolution of 64 columns)
   int H, W, cin, cout;
@@ -293,9 +271,7 @@ struct ds_vgg {
   ds_vgg_config cfg;
   bool bf16 = false;
   size_t esz = 4;
-  std::vector<std::string> names;
-  std::vector<int64_t> numel, off;
-  int64_t n_params = 0;
+  WeightTable w;
   VgConv conv[VG_NCONV];
   size_t fc1_off = 0, fc2_off = 0, wp_total = 0;     // packed-weight arena offsets
   int fc1_idx = 0, fc2_idx = 0;
@@ -317,16 +293,10 @@ void vg_free(ds_vgg* h) {
   for (void* b : bufs) cudaFree(b);
 }
 
-void add_name(ds_vgg* h, const std::string& n, int64_t numel) {
-  h->names.push_back(n);
-  h->numel.push_back(numel);
-  h->off.push_back(h->n_params);
-  h->n_params += numel;
-}
 
 bool encode(CUtensorMap* map, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
             const cuuint32_t* box, char* err, int err_len) {
-  PFN_encodeTiled enc = vg_encode();
+  const auto enc = tc_encode_tiled();
   if (!enc) {
     snprintf(err, err_len, "cuTensorMapEncodeTiled unavailable");
     return false;
@@ -412,25 +382,11 @@ int vg_pass_bf16(ds_vgg* h, int B, float* feat, cudaStream_t s) {
   int e = launch_gemm_tc(h->fc1, B, s);
   if (e) return fail(DS_ERR_CUDA, "vgg16: fc1 GEMM failed: %s", cudaGetErrorString((cudaError_t)e));
   const int64_t n = (int64_t)B * DS_VGG_FEATURES;
-  k_vgg_fill_bias<<<blocks(n, 256), 256, 0, s>>>(h->bias + h->fc2_b, feat, DS_VGG_FEATURES, n);
+  k_vgg_fill_bias<<<ceil_div(n, 256), 256, 0, s>>>(h->bias + h->fc2_b, feat, DS_VGG_FEATURES, n);
   tc_plan_set_atomic_out(h->fc2, feat, DS_VGG_FEATURES, 1);
   e = launch_gemm_tc(h->fc2, B, s);
   if (e) return fail(DS_ERR_CUDA, "vgg16: fc2 GEMM failed: %s", cudaGetErrorString((cudaError_t)e));
   return 0;
-}
-
-void simt(const float* a, int K, const float* w, const float* bias, float* d, int M, int N, int act, cudaStream_t s) {
-  constexpr int CHUNK = 32768 * 64;      // gridDim.y of the SIMT GEMM (64 rows per CTA row) stays below 65535
-  for (int m0 = 0; m0 < M; m0 += CHUNK) {
-    GemmArgs g;
-    memset(&g, 0, sizeof g);
-    g.a0 = a + (size_t)m0 * K; g.lda0 = K; g.k0 = K;
-    g.w = w; g.ldw = K;
-    g.bias = bias;
-    g.d = d + (size_t)m0 * N; g.ldd = N;
-    g.M = std::min(CHUNK, M - m0); g.N = N; g.act = act;
-    launch_gemm_simt<float>(g, true, s);
-  }
 }
 
 int vg_pass_fp32(ds_vgg* h, int B, float* feat, cudaStream_t s) {
@@ -440,17 +396,18 @@ int vg_pass_fp32(ds_vgg* h, int B, float* feat, cudaStream_t s) {
     float* out = (float*)h->act[l & 1];
     launch_re_im2col<float>(x, c.g, B, (float*)h->cols, s);
     const int M = B * c.H * c.W;
-    simt((const float*)h->cols, c.g.Kp, (const float*)h->wp + c.wp_off, h->bias + c.b_off, c.pool ? (float*)h->z : out,
-         M, c.cout, ACT_RELU, s);
+    launch_gemm_simt_chunked((const float*)h->cols, c.g.Kp, (const float*)h->wp + c.wp_off, h->bias + c.b_off,
+                             c.pool ? (float*)h->z : out, c.cout, M, c.cout, ACT_RELU, s);
     if (c.pool) {
       const int64_t n = (int64_t)B * (c.H / 2) * (c.W / 2) * c.cout;
-      k_vgg_pool<float><<<blocks(n, 256), 256, 0, s>>>((const float*)h->z, out, c.cout, c.H, c.W, n);
+      k_vgg_pool<float><<<ceil_div(n, 256), 256, 0, s>>>((const float*)h->z, out, c.cout, c.H, c.W, n);
     }
     x = out;
   }
-  simt(x, VG_FC1_K, (const float*)h->wp + h->fc1_off, h->bias + h->fc1_b, (float*)h->h1, B, DS_VGG_FEATURES, ACT_RELU, s);
-  simt((const float*)h->h1, DS_VGG_FEATURES, (const float*)h->wp + h->fc2_off, h->bias + h->fc2_b, feat, B,
-       DS_VGG_FEATURES, ACT_NONE, s);
+  launch_gemm_simt_chunked(x, VG_FC1_K, (const float*)h->wp + h->fc1_off, h->bias + h->fc1_b, (float*)h->h1,
+                           DS_VGG_FEATURES, B, DS_VGG_FEATURES, ACT_RELU, s);
+  launch_gemm_simt_chunked((const float*)h->h1, DS_VGG_FEATURES, (const float*)h->wp + h->fc2_off, h->bias + h->fc2_b,
+                           feat, DS_VGG_FEATURES, B, DS_VGG_FEATURES, ACT_NONE, s);
   CK(cudaGetLastError());
   return 0;
 }
@@ -506,18 +463,7 @@ extern "C" int ds_vgg_create(const ds_vgg_config* cfg, ds_vgg** out) {
     return fail(DS_ERR_INVALID, "vgg16: precision %d unknown", cfg->precision);
   if (cfg->capacity < 1 || cfg->capacity > 256)
     return fail(DS_ERR_INVALID, "vgg16: capacity %d outside [1, 256]", cfg->capacity);
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
-  if (cfg->device < 0 || cfg->device >= ndev) return fail(DS_ERR_INVALID, "device %d out of range", cfg->device);
-  CK(cudaSetDevice(cfg->device));
-  cudaDeviceProp prop;
-  CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 9)
-    return fail(DS_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major,
-                prop.minor);
+  if (const int rc = open_device(cfg->device)) return rc;
   if (cfg->precision == DS_PREC_BF16) {
     const int rc = vg_set_attrs();
     if (rc) return rc;
@@ -535,18 +481,18 @@ extern "C" int ds_vgg_create(const ds_vgg_config* cfg, ds_vgg** out) {
     h->wp_total += (size_t)c.cout * c.g.Kp;
     c.b_off = b_total;
     b_total += c.cout;
-    c.w_idx = int(h->names.size());
+    c.w_idx = int(h->w.names.size());
     const std::string pre = "features." + std::to_string(kFeatIdx[l]);
-    add_name(h, pre + ".weight", (int64_t)c.cout * c.cin * 9);
-    add_name(h, pre + ".bias", c.cout);
+    h->w.add(pre + ".weight", (int64_t)c.cout * c.cin * 9);
+    h->w.add(pre + ".bias", c.cout);
     if (c.pool) H /= 2;
   }
-  h->fc1_idx = int(h->names.size());
-  add_name(h, "classifier.0.weight", (int64_t)DS_VGG_FEATURES * VG_FC1_K);
-  add_name(h, "classifier.0.bias", DS_VGG_FEATURES);
-  h->fc2_idx = int(h->names.size());
-  add_name(h, "classifier.3.weight", (int64_t)DS_VGG_FEATURES * DS_VGG_FEATURES);
-  add_name(h, "classifier.3.bias", DS_VGG_FEATURES);
+  h->fc1_idx = int(h->w.names.size());
+  h->w.add("classifier.0.weight", (int64_t)DS_VGG_FEATURES * VG_FC1_K);
+  h->w.add("classifier.0.bias", DS_VGG_FEATURES);
+  h->fc2_idx = int(h->w.names.size());
+  h->w.add("classifier.3.weight", (int64_t)DS_VGG_FEATURES * DS_VGG_FEATURES);
+  h->w.add("classifier.3.bias", DS_VGG_FEATURES);
   h->fc1_off = h->wp_total;
   h->wp_total += (size_t)DS_VGG_FEATURES * VG_FC1_K;
   h->fc2_off = h->wp_total;
@@ -597,40 +543,37 @@ extern "C" int ds_vgg_destroy(ds_vgg* h) {
 
 extern "C" int ds_vgg_expected_weight_count(ds_vgg* h) {
   if (!h) return fail(DS_ERR_INVALID, "null handle");
-  return int(h->names.size());
+  return h->w.count();
 }
 
 extern "C" int ds_vgg_expected_weight(ds_vgg* h, int index, const char** name, int64_t* numel) {
-  if (!h || !name || !numel) return fail(DS_ERR_INVALID, "null argument");
-  if (index < 0 || index >= (int)h->names.size()) return fail(DS_ERR_INVALID, "weight index %d out of range", index);
-  *name = h->names[index].c_str();
-  *numel = h->numel[index];
-  return 0;
+  if (!h) return fail(DS_ERR_INVALID, "null argument");
+  return h->w.get(index, name, numel);
 }
 
 extern "C" int ds_vgg_set_weights(ds_vgg* h, const float* flat_params_dev, int64_t count, void* stream) {
   if (!h || !flat_params_dev) return fail(DS_ERR_INVALID, "null argument");
-  if (count != h->n_params)
-    return fail(DS_ERR_INVALID, "vgg16: %lld parameters given, %lld expected", (long long)count, (long long)h->n_params);
+  if (count != h->w.total)
+    return fail(DS_ERR_INVALID, "vgg16: %lld parameters given, %lld expected", (long long)count, (long long)h->w.total);
   CK(cudaSetDevice(h->cfg.device));
   cudaStream_t s = (cudaStream_t)stream;
   const float* p = flat_params_dev;
   for (int l = 0; l < VG_NCONV; ++l) {
     const VgConv& c = h->conv[l];
-    if (h->bf16) k_vgg_pack_conv<bf16><<<c.cout, 256, 0, s>>>(p + h->off[c.w_idx], c.cin, c.g.Kp, (bf16*)h->wp + c.wp_off);
-    else k_vgg_pack_conv<float><<<c.cout, 256, 0, s>>>(p + h->off[c.w_idx], c.cin, c.g.Kp, (float*)h->wp + c.wp_off);
-    CK(cudaMemcpyAsync(h->bias + c.b_off, p + h->off[c.w_idx + 1], c.cout * 4, cudaMemcpyDeviceToDevice, s));
+    if (h->bf16) k_vgg_pack_conv<bf16><<<c.cout, 256, 0, s>>>(p + h->w.off[c.w_idx], c.cin, c.g.Kp, (bf16*)h->wp + c.wp_off);
+    else k_vgg_pack_conv<float><<<c.cout, 256, 0, s>>>(p + h->w.off[c.w_idx], c.cin, c.g.Kp, (float*)h->wp + c.wp_off);
+    CK(cudaMemcpyAsync(h->bias + c.b_off, p + h->w.off[c.w_idx + 1], c.cout * 4, cudaMemcpyDeviceToDevice, s));
   }
   if (h->bf16) {
-    k_vgg_pack_fc<bf16><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->off[h->fc1_idx], VG_FC1_K, 1, (bf16*)h->wp + h->fc1_off);
-    k_vgg_pack_fc<bf16><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->off[h->fc2_idx], DS_VGG_FEATURES, 0, (bf16*)h->wp + h->fc2_off);
+    k_vgg_pack_fc<bf16><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->w.off[h->fc1_idx], VG_FC1_K, 1, (bf16*)h->wp + h->fc1_off);
+    k_vgg_pack_fc<bf16><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->w.off[h->fc2_idx], DS_VGG_FEATURES, 0, (bf16*)h->wp + h->fc2_off);
   } else {
-    k_vgg_pack_fc<float><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->off[h->fc1_idx], VG_FC1_K, 1, (float*)h->wp + h->fc1_off);
-    k_vgg_pack_fc<float><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->off[h->fc2_idx], DS_VGG_FEATURES, 0,
+    k_vgg_pack_fc<float><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->w.off[h->fc1_idx], VG_FC1_K, 1, (float*)h->wp + h->fc1_off);
+    k_vgg_pack_fc<float><<<DS_VGG_FEATURES, 256, 0, s>>>(p + h->w.off[h->fc2_idx], DS_VGG_FEATURES, 0,
                                                          (float*)h->wp + h->fc2_off);
   }
-  CK(cudaMemcpyAsync(h->bias + h->fc1_b, p + h->off[h->fc1_idx + 1], DS_VGG_FEATURES * 4, cudaMemcpyDeviceToDevice, s));
-  CK(cudaMemcpyAsync(h->bias + h->fc2_b, p + h->off[h->fc2_idx + 1], DS_VGG_FEATURES * 4, cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(h->bias + h->fc1_b, p + h->w.off[h->fc1_idx + 1], DS_VGG_FEATURES * 4, cudaMemcpyDeviceToDevice, s));
+  CK(cudaMemcpyAsync(h->bias + h->fc2_b, p + h->w.off[h->fc2_idx + 1], DS_VGG_FEATURES * 4, cudaMemcpyDeviceToDevice, s));
   CK(cudaGetLastError());
   h->weights_set = true;
   return 0;
@@ -649,8 +592,8 @@ extern "C" int ds_vgg_features(ds_vgg* h, const float* images_dev, int32_t batch
   for (int b0 = 0; b0 < batch; b0 += h->cfg.capacity) {
     const int B = std::min(h->cfg.capacity, batch - b0);
     const int64_t n = (int64_t)B * VG_IMG * VG_IMG * 3;
-    if (h->bf16) k_vgg_pack<bf16><<<blocks(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, height, width, (bf16*)h->x0, n);
-    else k_vgg_pack<float><<<blocks(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, height, width, (float*)h->x0, n);
+    if (h->bf16) k_vgg_pack<bf16><<<ceil_div(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, height, width, (bf16*)h->x0, n);
+    else k_vgg_pack<float><<<ceil_div(n, 256), 256, 0, s>>>(images_dev + b0 * img_n, height, width, (float*)h->x0, n);
     float* feat = features_dev + (int64_t)b0 * DS_VGG_FEATURES;
     const int rc = h->bf16 ? vg_pass_bf16(h, B, feat, s) : vg_pass_fp32(h, B, feat, s);
     if (rc) return rc;
@@ -669,11 +612,7 @@ extern "C" int ds_vgg_test_conv(const float* in_dev, int32_t batch, int32_t heig
     return fail(DS_ERR_INVALID, "vgg16 conv: cin %d must be 3 or a multiple of 64, cout %d 64 or a multiple of 128",
                 cin, cout);
   if (pool && (height % 2 || width % 2)) return fail(DS_ERR_INVALID, "vgg16 conv: pooled sides must be even");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return fail(DS_ERR_NO_DEVICE, "no CUDA device: diffuscene_b200 has no CPU fallback");
-  }
+  if (const int rc = require_device()) return rc;
   int rc = vg_set_attrs();
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
@@ -693,7 +632,7 @@ extern "C" int ds_vgg_test_conv(const float* in_dev, int32_t batch, int32_t heig
   rc = conv_maps(c, cin == 3 ? (const void*)cols : (const void*)x, wp, batch, 0);
   if (!rc) {
     conv_fwd_bf16(c, y, bias_dev, batch, s);
-    k_vgg_bf16_to_f32<<<blocks(n_out, 256), 256, 0, s>>>(y, out_dev, n_out);
+    launch_widen_bf16(y, out_dev, n_out, s);
   }
   cudaFreeAsync(x, s);
   cudaFreeAsync(wp, s);

@@ -21,10 +21,6 @@ LOSS_KEYS = ["loss.bbox", "loss.trans", "loss.size", "loss.angle", "loss.class",
              "loss.liou", "loss.bbox_iou"]
 
 
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
 class DenoiserEngine:
     """One Unet1D + diffusion schedule on one GPU (reference: DiffusionPoint, diffusion_ddpm.py:721-803)."""
 
@@ -67,17 +63,11 @@ class DenoiserEngine:
             pass
 
     def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return capi.stream(self.device)
 
     # ---- weights --------------------------------------------------------------------------------
     def expected_weights(self) -> List[tuple]:
-        n = self.lib.ds_expected_weight_count(self.h)
-        out = []
-        for i in range(n):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(self.lib.ds_expected_weight(self.h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
+        return capi.expected_weights(self.lib, "ds", self.h)
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], prefix: str = "diffusion.model."):
         """Load reference-format weights (keys as in the reference checkpoints) and commit them."""
@@ -105,7 +95,7 @@ class DenoiserEngine:
         capi.check(self.lib.ds_set_schedule(self.h, C.byref(s)))
         vt = [tables[f].detach().to(dtype=torch.float32, device="cpu").contiguous()
               for f in ("posterior_log_variance_clipped", "model_log_variance", "log_one_minus_alphas_cumprod")]
-        capi.check(self.lib.ds_set_vlb_schedule(self.h, tables.T, *[_ptr(a) for a in vt]))
+        capi.check(self.lib.ds_set_vlb_schedule(self.h, tables.T, *[capi.ptr(a) for a in vt]))
         self.tables = tables
 
     def set_context(self, context: torch.Tensor, shared: Optional[bool] = None):
@@ -122,7 +112,7 @@ class DenoiserEngine:
         # with torch on its default stream the library works on its own non-blocking stream, which does not wait for
         # the kernels that produced `context`: let them finish first
         torch.cuda.current_stream(self.device).synchronize()
-        capi.check(self.lib.ds_set_context(self.h, _ptr(ctx), batch, int(bool(shared)), self._stream()))
+        capi.check(self.lib.ds_set_context(self.h, capi.ptr(ctx), batch, int(bool(shared)), self._stream()))
         torch.cuda.current_stream(self.device).synchronize()
 
     def set_context_cross(self, cross: Optional[torch.Tensor]):
@@ -131,7 +121,7 @@ class DenoiserEngine:
             return
         c = cross.detach().to(device=self.device, dtype=torch.float32).contiguous()
         torch.cuda.current_stream(self.device).synchronize()      # as in set_context
-        capi.check(self.lib.ds_set_context_cross(self.h, _ptr(c), c.shape[0], c.shape[1], self._stream()))
+        capi.check(self.lib.ds_set_context_cross(self.h, capi.ptr(c), c.shape[0], c.shape[1], self._stream()))
         torch.cuda.current_stream(self.device).synchronize()
 
     # ---- denoiser -------------------------------------------------------------------------------
@@ -140,7 +130,8 @@ class DenoiserEngine:
         assert x_t.is_cuda and x_t.dtype == torch.float32 and t.dtype == torch.int64
         x_t, t = x_t.contiguous(), t.to(self.device).contiguous()
         out = torch.empty_like(x_t)
-        capi.check(self.lib.ds_denoise_forward(self.h, _ptr(x_t), _ptr(t), _ptr(out), x_t.shape[0], self._stream()))
+        capi.check(self.lib.ds_denoise_forward(self.h, capi.ptr(x_t), capi.ptr(t), capi.ptr(out), x_t.shape[0],
+                                               self._stream()))
         return out
 
     def forward_host(self, x_t: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
@@ -148,7 +139,7 @@ class DenoiserEngine:
         x_t = x_t.detach().to("cpu", torch.float32).contiguous()
         t = t.detach().to("cpu", torch.int64).contiguous()
         out = torch.empty_like(x_t)
-        capi.check(self.lib.ds_denoise_forward_host(self.h, _ptr(x_t), _ptr(t), _ptr(out), x_t.shape[0]))
+        capi.check(self.lib.ds_denoise_forward_host(self.h, capi.ptr(x_t), capi.ptr(t), capi.ptr(out), x_t.shape[0]))
         return out
 
     # ---- sampling -------------------------------------------------------------------------------
@@ -201,23 +192,24 @@ class DenoiserEngine:
         torch.cuda.current_stream(dev).synchronize()
         if host_output:
             out = torch.empty((batch, self.num_objects, self.d), dtype=torch.float32).pin_memory()
-            capi.check(self.lib.ds_sample_loop_host(self.h, C.byref(a), _ptr(out)))
+            capi.check(self.lib.ds_sample_loop_host(self.h, C.byref(a), capi.ptr(out)))
         else:
             out = torch.empty((batch, self.num_objects, self.d), device=dev, dtype=torch.float32)
-            capi.check(self.lib.ds_sample_loop(self.h, C.byref(a), _ptr(out), None))
+            capi.check(self.lib.ds_sample_loop(self.h, C.byref(a), capi.ptr(out), None))
         return (out, traj) if traj is not None else out
 
     def p_sample_step(self, x_t: torch.Tensor, t: torch.Tensor, noise: torch.Tensor, clip_denoised: bool):
         x_t, t, noise = x_t.contiguous(), t.to(self.device).contiguous(), noise.to(self.device).contiguous()
         out = torch.empty_like(x_t)
-        capi.check(self.lib.ds_p_sample_step(self.h, _ptr(x_t), _ptr(t), _ptr(noise), int(clip_denoised), _ptr(out),
-                                             x_t.shape[0], self._stream()))
+        capi.check(self.lib.ds_p_sample_step(self.h, capi.ptr(x_t), capi.ptr(t), capi.ptr(noise), int(clip_denoised),
+                                             capi.ptr(out), x_t.shape[0], self._stream()))
         return out
 
     def q_sample(self, x0: torch.Tensor, t: torch.Tensor, noise: torch.Tensor):
         x0, t, noise = x0.contiguous(), t.to(self.device).contiguous(), noise.contiguous()
         out = torch.empty_like(x0)
-        capi.check(self.lib.ds_q_sample(self.h, _ptr(x0), _ptr(t), _ptr(noise), _ptr(out), x0.shape[0], self._stream()))
+        capi.check(self.lib.ds_q_sample(self.h, capi.ptr(x0), capi.ptr(t), capi.ptr(noise), capi.ptr(out), x0.shape[0],
+                                        self._stream()))
         return out
 
     def p_losses(self, x0: torch.Tensor, t: torch.Tensor, noise: torch.Tensor, loss_separate: bool, loss_iou: bool,
@@ -230,8 +222,8 @@ class DenoiserEngine:
         barr = None
         if bounds is not None:
             barr = (C.c_float * 12)(*[float(v) for v in bounds])
-        capi.check(self.lib.ds_p_losses(self.h, _ptr(x0), _ptr(t), _ptr(noise), int(loss_separate), int(loss_iou),
-                                        barr, _ptr(losses), _ptr(ld), B, self._stream()))
+        capi.check(self.lib.ds_p_losses(self.h, capi.ptr(x0), capi.ptr(t), capi.ptr(noise), int(loss_separate),
+                                        int(loss_iou), barr, capi.ptr(losses), capi.ptr(ld), B, self._stream()))
         return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}
 
     # ---- variational bound ----------------------------------------------------------------------
@@ -255,7 +247,7 @@ class DenoiserEngine:
         mse = None if prior_only else torch.empty((B, T), device=dev, dtype=torch.float32)
         prior = torch.empty(B, device=dev, dtype=torch.float32)
         torch.cuda.current_stream(dev).synchronize()
-        capi.check(self.lib.ds_vlb_loop(self.h, C.byref(a), _ptr(vb), _ptr(mse), _ptr(prior), None))
+        capi.check(self.lib.ds_vlb_loop(self.h, C.byref(a), capi.ptr(vb), capi.ptr(mse), capi.ptr(prior), None))
         return vb, mse, prior
 
     # ---- native training ------------------------------------------------------------------------
@@ -284,15 +276,15 @@ class DenoiserEngine:
         ld = torch.empty(9, device=self.device, dtype=torch.float32)
         dctx = torch.empty_like(ctx) if (want_dcontext and flat_grads is not None) else None
         barr = None if bounds is None else (C.c_float * 12)(*[float(v) for v in bounds])
-        args = (self.h, _ptr(flat_params), _ptr(x0), _ptr(t), _ptr(noise), _ptr(ctx), 0 if shared else B,
-                int(bool(shared)), int(loss_separate), int(loss_iou), barr, float(grad_scale), _ptr(losses), _ptr(ld),
-                _ptr(flat_grads), _ptr(dctx))
+        args = (self.h, capi.ptr(flat_params), capi.ptr(x0), capi.ptr(t), capi.ptr(noise), capi.ptr(ctx),
+                0 if shared else B, int(bool(shared)), int(loss_separate), int(loss_iou), barr, float(grad_scale),
+                capi.ptr(losses), capi.ptr(ld), capi.ptr(flat_grads), capi.ptr(dctx))
         if cross is None:
             capi.check(self.lib.ds_train_step(*args, B, self._stream()))
             return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}, dctx
         xc = cross.detach().to(self.device, torch.float32).contiguous()
         dxc = torch.empty_like(xc) if (want_dcross and flat_grads is not None) else None
-        capi.check(self.lib.ds_train_step_cross(*args, _ptr(xc), xc.shape[1], _ptr(dxc), B, self._stream()))
+        capi.check(self.lib.ds_train_step_cross(*args, capi.ptr(xc), xc.shape[1], capi.ptr(dxc), B, self._stream()))
         return losses, {k: ld[i] for i, k in enumerate(LOSS_KEYS)}, dctx, dxc
 
     def train_set_buckets(self, bounds: Sequence[int], events: Sequence["torch.cuda.Event"]):
@@ -318,7 +310,7 @@ class DenoiserEngine:
         r, w = C.c_int32(), C.c_int32()
         capi.check(self.lib.ds_train_read(self.h, kind, int(index), None, 0, C.byref(r), C.byref(w), self._stream()))
         out = torch.empty(r.value * w.value, device=self.device, dtype=torch.float32)
-        capi.check(self.lib.ds_train_read(self.h, kind, int(index), _ptr(out), out.numel(), C.byref(r), C.byref(w),
+        capi.check(self.lib.ds_train_read(self.h, kind, int(index), capi.ptr(out), out.numel(), C.byref(r), C.byref(w),
                                           self._stream()))
         return out[: r.value * w.value].view(r.value, w.value)
 
@@ -330,7 +322,7 @@ class DenoiserEngine:
         cap = 1 << 26
         buf = torch.empty(cap, dtype=torch.float32)
         r, w = C.c_int32(), C.c_int32()
-        capi.check(self.lib.ds_read_tap(self.h, name.encode(), _ptr(buf), cap, C.byref(r), C.byref(w)))
+        capi.check(self.lib.ds_read_tap(self.h, name.encode(), capi.ptr(buf), cap, C.byref(r), C.byref(w)))
         return buf[: r.value * w.value].reshape(r.value, w.value)[:rows].clone()
 
     def launch_count(self) -> int:

@@ -17,7 +17,6 @@ to the scene unless --without_floor is not part of the statistics, and the mesh-
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -78,14 +77,6 @@ def footprint_table(footprints: Sequence) -> Dict[str, np.ndarray]:
     return {"hull_offsets": offsets, "hull_xz": hull, "raw_half": half, "raw_aabb": aabb}
 
 
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream(dev: torch.device):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 def scene_boxes(translations: torch.Tensor, sizes: torch.Tensor, angles: torch.Tensor,
                 model_index: Optional[torch.Tensor] = None, catalog: Optional[ObjectCatalog] = None) -> torch.Tensor:
     """World-space translations / sizes [..., 3] and angles [..., 1] (after post_process_batch), catalogue indices
@@ -109,9 +100,10 @@ def scene_boxes(translations: torch.Tensor, sizes: torch.Tensor, angles: torch.T
     out = torch.empty(Q, 6, dtype=torch.float64, device=dev)
     lib = capi.load()
     capi.check(lib.ds_scene_boxes(
-        _ptr(t), _ptr(s), _ptr(a), _ptr(idx), Q, _ptr(fp and fp["hull_offsets"]), _ptr(fp and fp["hull_xz"]),
-        0 if fp is None else fp["hull_xz"].shape[0], _ptr(fp and fp["raw_half"]), _ptr(fp and fp["raw_aabb"]),
-        0 if fp is None else fp["raw_half"].shape[0], _ptr(out), _stream(dev)))
+        capi.ptr(t), capi.ptr(s), capi.ptr(a), capi.ptr(idx), Q, capi.ptr(fp and fp["hull_offsets"]),
+        capi.ptr(fp and fp["hull_xz"]),
+        0 if fp is None else fp["hull_xz"].shape[0], capi.ptr(fp and fp["raw_half"]), capi.ptr(fp and fp["raw_aabb"]),
+        0 if fp is None else fp["raw_half"].shape[0], capi.ptr(out), capi.stream(dev)))
     return out.reshape(shape + (6,))
 
 
@@ -136,8 +128,8 @@ def scene_stats(bounds: torch.Tensor, class_index: torch.Tensor, keep: Optional[
         out["pair_iou"] = torch.empty(B, N, N, device=dev)
     lib = capi.load()
     capi.check(lib.ds_scene_stats(
-        _ptr(bx), _ptr(kp), _ptr(cl), _ptr(mi), B, N, *[_ptr(out[k]) for k in STAT_KEYS], _ptr(out.get("pair_iou")),
-        _stream(dev)))
+        capi.ptr(bx), capi.ptr(kp), capi.ptr(cl), capi.ptr(mi), B, N, *[capi.ptr(out[k]) for k in STAT_KEYS],
+        capi.ptr(out.get("pair_iou")), capi.stream(dev)))
     return out
 
 

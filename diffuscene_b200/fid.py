@@ -81,7 +81,7 @@ def _files(src: Union[str, Sequence[str]]) -> List[str]:
 
 # ---- features ---------------------------------------------------------------------------------------------------
 
-class InceptionFeatures:
+class InceptionFeatures(capi.FeatureNet):
     """pool3 features of the FID Inception-v3 on the device.
 
     precision "fp32" (default): im2col + exact SIMT GEMMs, the detector's fp32 features up to summation order;
@@ -89,90 +89,13 @@ class InceptionFeatures:
     Inception state dict (torchvision `Inception3` key names), a file holding one, or the module itself.
     Call with fp32 [B, 3, 299, 299] in [0, 255] (any device, already clean-resized); returns fp32 [B, 2048] on the
     device."""
-
-    def __init__(self, state_dict_or_path: Union[str, dict, torch.nn.Module], precision: str = "fp32",
-                 capacity: Optional[int] = None, device: int = 0):
-        if precision not in ("bf16", "fp32"):
-            raise ValueError("precision must be 'bf16' or 'fp32', not %r" % (precision,))
-        sd = state_dict_or_path
-        if isinstance(sd, (str, os.PathLike)):
-            sd = torch.load(sd, map_location="cpu", weights_only=True)
-        elif isinstance(sd, torch.nn.Module):
-            sd = sd.state_dict()
-        if not isinstance(sd, dict):
-            raise TypeError("Inception weights must be a state dict, a state-dict file or a module, not %s"
-                            % type(state_dict_or_path).__name__)
-        if not torch.cuda.is_available():
-            raise RuntimeError("InceptionFeatures needs a CUDA device: diffuscene_b200 has no CPU fallback")
-        self.lib = capi.load()
-        self.device = torch.device("cuda", device)
-        cfg = capi.DsInceptionConfig()
-        cfg.precision = capi.DS_PREC_BF16 if precision == "bf16" else capi.DS_PREC_FP32
-        cfg.capacity = capacity or (64 if precision == "bf16" else 8)
-        cfg.device = device
-        self.capacity = cfg.capacity
-        self.precision = precision
-        self._h = C.c_void_p()
-        capi.check(self.lib.ds_inception_create(C.byref(cfg), C.byref(self._h)))
-        names = expected_weights(self.lib, self._h)
-        missing = [n for n, _ in names if n not in sd]
-        if missing:
-            self.close()
-            raise KeyError("Inception state dict lacks %s" % ", ".join(missing))
-        for n, numel in names:
-            if sd[n].numel() != numel:
-                self.close()
-                raise ValueError("%s has %d elements, expected %d" % (n, sd[n].numel(), numel))
-        flat = torch.cat([sd[n].reshape(-1).float() for n, _ in names]).to(self.device)
-        stream = torch.cuda.current_stream(self.device)
-        capi.check(self.lib.ds_inception_set_weights(self._h, C.c_void_p(flat.data_ptr()), flat.numel(),
-                                                     C.c_void_p(stream.cuda_stream)))
-        stream.synchronize()
-
-    def __call__(self, images: torch.Tensor) -> torch.Tensor:
-        if images.dim() != 4 or images.shape[1] != 3:
-            raise ValueError("images must be [B, 3, 299, 299], got %s" % (tuple(images.shape),))
-        x = images.to(self.device, torch.float32).contiguous()
-        out = torch.empty(x.shape[0], FEATURES, device=self.device, dtype=torch.float32)
-        if x.shape[0] == 0:
-            return out
-        stream = torch.cuda.current_stream(self.device)
-        capi.check(self.lib.ds_inception_features(self._h, C.c_void_p(x.data_ptr()), x.shape[0], x.shape[2],
-                                                  x.shape[3], C.c_void_p(out.data_ptr()),
-                                                  C.c_void_p(stream.cuda_stream)))
-        return out
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.ds_inception_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    prefix, config, features = "ds_inception", capi.DsInceptionConfig, FEATURES
+    name, image_shape, cuda_guard = "Inception", "[B, 3, 299, 299]", True
 
 
 def expected_weights(lib=None, h=None) -> List[tuple]:
     """(name, numel) of the flat parameter buffer, torchvision state-dict order (needs a device for the handle)."""
-    lib = lib or capi.load()
-    own = h is None
-    if own:
-        cfg = capi.DsInceptionConfig()
-        cfg.precision, cfg.capacity = capi.DS_PREC_FP32, 1
-        h = C.c_void_p()
-        capi.check(lib.ds_inception_create(C.byref(cfg), C.byref(h)))
-    try:
-        out = []
-        for i in range(capi.check(lib.ds_inception_expected_weight_count(h))):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(lib.ds_inception_expected_weight(h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
-    finally:
-        if own:
-            lib.ds_inception_destroy(h)
+    return InceptionFeatures.inventory(lib, h)
 
 
 def folder_features(files: Union[str, Sequence[str]], model: InceptionFeatures, batch_size: int = 32,
@@ -190,10 +113,6 @@ def folder_features(files: Union[str, Sequence[str]], model: InceptionFeatures, 
 
 # ---- statistics and distances -----------------------------------------------------------------------------------
 
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _dev32(x) -> torch.Tensor:
     t = x if isinstance(x, torch.Tensor) else torch.as_tensor(np.asarray(x, np.float32))
     return t.to("cuda", torch.float32).contiguous()
@@ -209,7 +128,7 @@ def feature_stats(feats) -> Tuple[np.ndarray, np.ndarray]:
     mu = torch.empty(d, device=f.device, dtype=torch.float64)
     sigma = torch.empty(d, d, device=f.device, dtype=torch.float64)
     capi.check(capi.load().ds_feature_stats(C.c_void_p(f.data_ptr()), n, d, C.c_void_p(mu.data_ptr()),
-                                            C.c_void_p(sigma.data_ptr()), _stream()))
+                                            C.c_void_p(sigma.data_ptr()), capi.stream()))
     return mu.cpu().numpy(), sigma.cpu().numpy()
 
 
@@ -265,7 +184,7 @@ def kid_terms(feats_real, feats_fake, idx_fake, idx_real) -> np.ndarray:
     terms = torch.empty(subsets, device="cuda", dtype=torch.float64)
     capi.check(capi.load().ds_kid_terms(C.c_void_p(r.data_ptr()), r.shape[0], C.c_void_p(f.data_ptr()), f.shape[0],
                                         r.shape[1], C.c_void_p(ix.data_ptr()), C.c_void_p(iy.data_ptr()), subsets, m,
-                                        C.c_void_p(terms.data_ptr()), _stream()))
+                                        C.c_void_p(terms.data_ptr()), capi.stream()))
     return terms.cpu().numpy()
 
 

@@ -11,13 +11,12 @@ The VGG16 weights are never downloaded: pass a torchvision state-dict file or di
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 import random
 from collections import namedtuple
 from concurrent.futures import ThreadPoolExecutor
 from glob import glob
-from typing import List, Optional, Sequence, Union
+from typing import List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -52,7 +51,7 @@ def find_weights(path: Optional[str] = None) -> str:
 
 # ---- features ---------------------------------------------------------------------------------------------------
 
-class VGG16Features:
+class VGG16Features(capi.FeatureNet):
     """classifier[:4](features(x).view(-1, 25088)) of torchvision vgg16 on the device.
 
     precision "fp32" (default): im2col + exact SIMT GEMMs, the reference's fp32 features up to summation order;
@@ -61,88 +60,13 @@ class VGG16Features:
     torchvision vgg16 state dict, a file holding one, or the vgg16 nn.Module itself.
     Call with a normalised fp32 tensor [B, 3, H, W] (any device); returns fp32 [B, 4096] on the device.  Inputs other
     than 224 x 224 are resized with F.interpolate's nearest pixel choice, as the reference's extract_features."""
-
-    def __init__(self, state_dict_or_path: Union[str, dict, torch.nn.Module], precision: str = "fp32",
-                 capacity: Optional[int] = None,
-                 device: int = 0):
-        if precision not in ("bf16", "fp32"):
-            raise ValueError("precision must be 'bf16' or 'fp32', not %r" % (precision,))
-        sd = state_dict_or_path
-        if isinstance(sd, str):
-            sd = torch.load(sd, map_location="cpu", weights_only=True)
-        elif isinstance(sd, torch.nn.Module):
-            sd = sd.state_dict()
-        if not isinstance(sd, dict):
-            raise TypeError("VGG16 weights must be a state dict, a state-dict file or a vgg16 module, not %s"
-                            % type(state_dict_or_path).__name__)
-        self.lib = capi.load()
-        self.device = torch.device("cuda", device)
-        cfg = capi.DsVggConfig()
-        cfg.precision = capi.DS_PREC_BF16 if precision == "bf16" else capi.DS_PREC_FP32
-        cfg.capacity = capacity or (64 if precision == "bf16" else 8)
-        cfg.device = device
-        self.capacity = cfg.capacity
-        self.precision = precision
-        self._h = C.c_void_p()
-        capi.check(self.lib.ds_vgg_create(C.byref(cfg), C.byref(self._h)))
-        names = expected_weights(self.lib, self._h)
-        missing = [n for n, _ in names if n not in sd]
-        if missing:
-            self.close()
-            raise KeyError("VGG16 state dict lacks %s" % ", ".join(missing))
-        for n, numel in names:
-            if sd[n].numel() != numel:
-                self.close()
-                raise ValueError("%s has %d elements, expected %d" % (n, sd[n].numel(), numel))
-        flat = torch.cat([sd[n].reshape(-1).float() for n, _ in names]).to(self.device)
-        stream = torch.cuda.current_stream(self.device)
-        capi.check(self.lib.ds_vgg_set_weights(self._h, C.c_void_p(flat.data_ptr()), flat.numel(),
-                                               C.c_void_p(stream.cuda_stream)))
-        stream.synchronize()
-
-    def __call__(self, images: torch.Tensor) -> torch.Tensor:
-        if images.dim() != 4 or images.shape[1] != 3:
-            raise ValueError("images must be [B, 3, H, W], got %s" % (tuple(images.shape),))
-        x = images.to(self.device, torch.float32).contiguous()
-        out = torch.empty(x.shape[0], 4096, device=self.device, dtype=torch.float32)
-        if x.shape[0] == 0:
-            return out
-        stream = torch.cuda.current_stream(self.device)
-        capi.check(self.lib.ds_vgg_features(self._h, C.c_void_p(x.data_ptr()), x.shape[0], x.shape[2], x.shape[3],
-                                            C.c_void_p(out.data_ptr()), C.c_void_p(stream.cuda_stream)))
-        return out
-
-    def close(self):
-        if getattr(self, "_h", None) and self._h.value:
-            self.lib.ds_vgg_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    prefix, config, features = "ds_vgg", capi.DsVggConfig, 4096
+    name, module = "VGG16", "a vgg16 module"
 
 
 def expected_weights(lib=None, h=None) -> List[tuple]:
     """(name, numel) of the flat parameter buffer, torchvision state-dict order (needs a device for the handle)."""
-    lib = lib or capi.load()
-    own = h is None
-    if own:
-        cfg = capi.DsVggConfig()
-        cfg.precision, cfg.capacity = capi.DS_PREC_FP32, 1
-        h = C.c_void_p()
-        capi.check(lib.ds_vgg_create(C.byref(cfg), C.byref(h)))
-    try:
-        out = []
-        for i in range(capi.check(lib.ds_vgg_expected_weight_count(h))):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(lib.ds_vgg_expected_weight(h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
-    finally:
-        if own:
-            lib.ds_vgg_destroy(h)
+    return VGG16Features.inventory(lib, h)
 
 
 def load_image(path: str) -> np.ndarray:
@@ -180,14 +104,6 @@ def _dev64(x) -> torch.Tensor:
     return t.to("cuda", torch.float64).contiguous()
 
 
-def _ptr(t: Optional[torch.Tensor]):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _warn_clamped(clamped: torch.Tensor):
     n = int(clamped.item())
     if n:
@@ -203,8 +119,8 @@ def compute_pairwise_distances(X, Y=None) -> np.ndarray:
         raise ValueError("feature sizes differ: %d and %d" % (x.shape[1], y.shape[1]))
     out = torch.empty(x.shape[0], y.shape[0], device="cuda", dtype=torch.float64)
     clamped = torch.zeros(1, device="cuda", dtype=torch.int64)
-    capi.check(lib.ds_manifold_distances(_ptr(x), x.shape[0], _ptr(y), y.shape[0], x.shape[1], _ptr(out),
-                                         _ptr(clamped), _stream()))
+    capi.check(lib.ds_manifold_distances(capi.ptr(x), x.shape[0], capi.ptr(y), y.shape[0], x.shape[1], capi.ptr(out),
+                                         capi.ptr(clamped), capi.stream()))
     _warn_clamped(clamped)
     return out.cpu().numpy()
 
@@ -224,7 +140,8 @@ def manifold_radii(features, k: int = 3) -> np.ndarray:
     x = _dev64(features)
     radii = torch.empty(x.shape[0], device="cuda", dtype=torch.float64)
     clamped = torch.zeros(1, device="cuda", dtype=torch.int64)
-    capi.check(lib.ds_manifold_radii(_ptr(x), x.shape[0], x.shape[1], int(k), _ptr(radii), _ptr(clamped), _stream()))
+    capi.check(lib.ds_manifold_radii(capi.ptr(x), x.shape[0], x.shape[1], int(k), capi.ptr(radii), capi.ptr(clamped),
+                                     capi.stream()))
     _warn_clamped(clamped)
     return radii.cpu().numpy()
 
@@ -243,8 +160,9 @@ def manifold_cover(manifold_ref: Manifold, feats_subject, radii_subject=None, wa
     r_cov = torch.empty(ref.shape[0], device="cuda", dtype=torch.uint8) if r_subj is not None else None
     real = torch.empty(subj.shape[0], device="cuda", dtype=torch.float64) if want_realism else None
     clamped = torch.zeros(1, device="cuda", dtype=torch.int64)
-    capi.check(lib.ds_manifold_cover(_ptr(ref), _ptr(r_ref), ref.shape[0], _ptr(subj), _ptr(r_subj), subj.shape[0],
-                                     ref.shape[1], _ptr(s_cov), _ptr(r_cov), _ptr(real), _ptr(clamped), _stream()))
+    capi.check(lib.ds_manifold_cover(capi.ptr(ref), capi.ptr(r_ref), ref.shape[0], capi.ptr(subj), capi.ptr(r_subj),
+                                     subj.shape[0],
+                                     ref.shape[1], capi.ptr(s_cov), capi.ptr(r_cov), capi.ptr(real), capi.ptr(clamped), capi.stream()))
     _warn_clamped(clamped)
     return (s_cov.cpu().numpy().astype(bool), None if r_cov is None else r_cov.cpu().numpy().astype(bool),
             None if real is None else real.cpu().numpy())

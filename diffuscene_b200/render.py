@@ -299,10 +299,6 @@ def choose_floor_textures(num_scenes: int, num_textures: int, seed: int = 0) -> 
 
 # ---- rendering --------------------------------------------------------------------------------------------------
 
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
 def render_scenes(catalog: MeshCatalog, translations, sizes, angles, model_index, class_index=None,
                   floors: Optional[Tuple[np.ndarray, np.ndarray]] = None, no_texture: bool = False,
                   white_background: bool = False, camera: Optional[Camera] = None, palette=None,
@@ -358,7 +354,7 @@ def render_scenes(catalog: MeshCatalog, translations, sizes, angles, model_index
     args.id_dev = None if ids is None else ids.data_ptr()
     cam = camera.struct()
     capi.check(catalog.lib.ds_render_scenes(catalog._h, C.byref(cam), C.byref(args),
-                                            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                            capi.stream(dev)))
     return (img, ids) if return_ids else img
 
 
@@ -497,9 +493,8 @@ def clean_resize(renders: torch.Tensor, size: int = 299) -> torch.Tensor:
     B, H, W, _ = x.shape
     hb, hk, vb, vk = _tables(H, W, size, size, "bicubic", False, x.device)
     out = torch.empty(B, 3, size, size, device=x.device, dtype=torch.float32)
-    capi.check(capi.load().ds_resize_f32(_ptr(x), B, H, W, size, size, _ptr(hb), _ptr(hk), hk.shape[1], _ptr(vb),
-                                         _ptr(vk), vk.shape[1], _ptr(out),
-                                         C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+    capi.check(capi.load().ds_resize_f32(capi.ptr(x), B, H, W, size, size, capi.ptr(hb), capi.ptr(hk), hk.shape[1],
+                                         capi.ptr(vb), capi.ptr(vk), vk.shape[1], capi.ptr(out), capi.stream(x.device)))
     return out
 
 
@@ -512,9 +507,8 @@ def ipr_resize(renders: torch.Tensor, size: int = 224) -> torch.Tensor:
     hb, hk, vb, vk = _tables(H, W, size, size, "bilinear", True, x.device)
     ms = (C.c_float * 6)(*IMAGENET_MEAN, *IMAGENET_STD)
     out = torch.empty(B, 3, size, size, device=x.device, dtype=torch.float32)
-    capi.check(capi.load().ds_resize_u8(_ptr(x), B, H, W, size, size, _ptr(hb), _ptr(hk), hk.shape[1], _ptr(vb),
-                                        _ptr(vk), vk.shape[1], ms, _ptr(out),
-                                        C.c_void_p(torch.cuda.current_stream(x.device).cuda_stream)))
+    capi.check(capi.load().ds_resize_u8(capi.ptr(x), B, H, W, size, size, capi.ptr(hb), capi.ptr(hk), hk.shape[1],
+                                        capi.ptr(vb), capi.ptr(vk), vk.shape[1], ms, capi.ptr(out), capi.stream(x.device)))
     return out
 
 

@@ -64,16 +64,7 @@ class RoomMaskEncoder:
         self.generation = 0      # bumped by every forward that keeps its activations
 
     def expected_weights(self) -> List[Tuple[str, int]]:
-        n = capi.check(self.lib.ds_room_enc_expected_weight_count(self.h))
-        out = []
-        for i in range(n):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(self.lib.ds_room_enc_expected_weight(self.h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return capi.expected_weights(self.lib, "ds_room_enc", self.h)
 
     def forward(self, flat: torch.Tensor, mask: torch.Tensor, keep: bool = False) -> torch.Tensor:
         cfg = self.cfg
@@ -83,7 +74,7 @@ class RoomMaskEncoder:
                                                                             tuple(mask.shape)))
         feat = torch.empty(mask.shape[0], 512, device=self.device, dtype=torch.float32)
         capi.check(self.lib.ds_room_enc_forward(self.h, C.c_void_p(flat.data_ptr()), C.c_void_p(mask.data_ptr()),
-                                                mask.shape[0], C.c_void_p(feat.data_ptr()), int(keep), self._stream()))
+                                                mask.shape[0], C.c_void_p(feat.data_ptr()), int(keep), capi.stream(self.device)))
         if keep:
             self.generation += 1
         return feat
@@ -91,7 +82,7 @@ class RoomMaskEncoder:
     def backward(self, dfeat: torch.Tensor, grads: torch.Tensor):
         dfeat = dfeat.to(self.device, torch.float32).contiguous()
         capi.check(self.lib.ds_room_enc_backward(self.h, C.c_void_p(dfeat.data_ptr()), C.c_void_p(grads.data_ptr()),
-                                                 self._stream()))
+                                                 capi.stream(self.device)))
 
     def read(self, kind, index: int = 0) -> torch.Tensor:
         """One array of the encoder's state (ds_room_enc_read), fp32 [rows, width] on the device: kind is a name of
@@ -99,10 +90,11 @@ class RoomMaskEncoder:
         if isinstance(kind, str):
             kind = capi.ROOM_ENC_STATE[kind]
         r, w = C.c_int32(), C.c_int32()
-        capi.check(self.lib.ds_room_enc_read(self.h, kind, int(index), None, 0, C.byref(r), C.byref(w), self._stream()))
+        capi.check(self.lib.ds_room_enc_read(self.h, kind, int(index), None, 0, C.byref(r), C.byref(w),
+                                             capi.stream(self.device)))
         out = torch.empty(r.value, w.value, device=self.device, dtype=torch.float32)
         capi.check(self.lib.ds_room_enc_read(self.h, kind, int(index), C.c_void_p(out.data_ptr()), out.numel(),
-                                             C.byref(r), C.byref(w), self._stream()))
+                                             C.byref(r), C.byref(w), capi.stream(self.device)))
         return out
 
     def close(self):

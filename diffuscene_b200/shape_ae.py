@@ -77,16 +77,7 @@ class ShapeAE:
         self._inject = None
 
     def expected_weights(self) -> List[Tuple[str, int]]:
-        n = capi.check(self.lib.ds_shape_ae_expected_weight_count(self.h))
-        out = []
-        for i in range(n):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(self.lib.ds_shape_ae_expected_weight(self.h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+        return capi.expected_weights(self.lib, "ds_shape_ae", self.h)
 
     def _points(self, points):
         points = points.to(self.device, torch.float32).contiguous()
@@ -101,9 +92,8 @@ class ShapeAE:
         lat = torch.empty(B, F, device=self.device)
         kl = torch.empty(B, device=self.device)
         rec = torch.empty(B, GRID_POINTS, 3, device=self.device)
-        ptr = lambda t: C.c_void_p(t.data_ptr())
-        capi.check(self.lib.ds_shape_ae_forward(self.h, ptr(flat), ptr(points), B, ptr(eps), int(train), int(keep),
-                                                ptr(lat), ptr(kl), ptr(rec), self._stream()))
+        capi.check(self.lib.ds_shape_ae_forward(self.h, capi.ptr(flat), capi.ptr(points), B, capi.ptr(eps), int(train),
+                                                int(keep), capi.ptr(lat), capi.ptr(kl), capi.ptr(rec), capi.stream(self.device)))
         return kl, lat, rec
 
     def train_step(self, flat, grads, points, eps, kl_weight: float) -> torch.Tensor:
@@ -111,9 +101,9 @@ class ShapeAE:
         points = self._points(points)
         eps = eps.to(self.device, torch.float32).contiguous()
         losses = torch.empty(3, device=self.device)
-        ptr = lambda t: C.c_void_p(t.data_ptr())
-        capi.check(self.lib.ds_shape_ae_train_step(self.h, ptr(flat), ptr(points), points.shape[0], ptr(eps),
-                                                   float(kl_weight), ptr(grads), ptr(losses), self._stream()))
+        capi.check(self.lib.ds_shape_ae_train_step(self.h, capi.ptr(flat), capi.ptr(points), points.shape[0],
+                                                   capi.ptr(eps), float(kl_weight), capi.ptr(grads), capi.ptr(losses),
+                                                   capi.stream(self.device)))
         return losses
 
     def set_knn(self, idx: Optional[torch.Tensor]):
@@ -124,7 +114,7 @@ class ShapeAE:
 
     def get_knn(self, batch: int) -> torch.Tensor:
         out = torch.empty(3, batch, self.cfg.num_points, 16, dtype=torch.int32, device=self.device)
-        capi.check(self.lib.ds_shape_ae_get_knn(self.h, C.c_void_p(out.data_ptr()), self._stream()))
+        capi.check(self.lib.ds_shape_ae_get_knn(self.h, C.c_void_p(out.data_ptr()), capi.stream(self.device)))
         return out
 
     def close(self):
@@ -307,9 +297,8 @@ def chamfer_3d(a, b):
     d2 = torch.empty(B, m, device=a.device)
     i1 = torch.empty(B, n, device=a.device, dtype=torch.int32)
     i2 = torch.empty(B, m, device=a.device, dtype=torch.int32)
-    ptr = lambda t: C.c_void_p(t.data_ptr())
-    capi.check(lib.ds_chamfer_forward(ptr(a), n, ptr(b), m, B, ptr(d1), ptr(d2), ptr(i1), ptr(i2),
-                                      C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream)))
+    capi.check(lib.ds_chamfer_forward(capi.ptr(a), n, capi.ptr(b), m, B, capi.ptr(d1), capi.ptr(d2), capi.ptr(i1),
+                                      capi.ptr(i2), capi.stream(a.device)))
     return d1, d2, i1, i2
 
 
@@ -330,11 +319,10 @@ class ChamferFunction(torch.autograd.Function):
         g2 = torch.zeros_like(b[..., 0]) if g2 is None else g2.contiguous()
         ga = torch.empty_like(a) if ctx.needs_input_grad[0] else None
         gb = torch.empty_like(b) if ctx.needs_input_grad[1] else None
-        ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())
         if ga is not None or gb is not None:
             capi.check(capi.load().ds_chamfer_backward(
-                ptr(a), a.shape[1], ptr(b), b.shape[1], a.shape[0], ptr(i1), ptr(i2), ptr(g1), ptr(g2), ptr(ga),
-                ptr(gb), C.c_void_p(torch.cuda.current_stream(a.device).cuda_stream)))
+                capi.ptr(a), a.shape[1], capi.ptr(b), b.shape[1], a.shape[0], capi.ptr(i1), capi.ptr(i2), capi.ptr(g1),
+                capi.ptr(g2), capi.ptr(ga), capi.ptr(gb), capi.stream(a.device)))
         return ga, gb
 
 

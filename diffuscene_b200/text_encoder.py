@@ -117,9 +117,6 @@ class BertTextEncoder:
         self.capacity = 0
         self._create(capacity)
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def _create(self, capacity: int):
         self.close()
         g = self.geometry
@@ -131,16 +128,10 @@ class BertTextEncoder:
         capi.check(self.lib.ds_text_enc_create(C.byref(cfg), C.byref(h)))
         self.h, self.capacity = h, capacity
         flat = self._flat_host.to(self.device)
-        capi.check(self.lib.ds_text_enc_set_weights(self.h, C.c_void_p(flat.data_ptr()), self._stream()))
+        capi.check(self.lib.ds_text_enc_set_weights(self.h, C.c_void_p(flat.data_ptr()), capi.stream(self.device)))
 
     def expected_weights(self) -> List[Tuple[str, int]]:
-        n = capi.check(self.lib.ds_text_enc_expected_weight_count(self.h))
-        out = []
-        for i in range(n):
-            name, numel = C.c_char_p(), C.c_int64()
-            capi.check(self.lib.ds_text_enc_expected_weight(self.h, i, C.byref(name), C.byref(numel)))
-            out.append((name.value.decode(), numel.value))
-        return out
+        return capi.expected_weights(self.lib, "ds_text_enc", self.h)
 
     def __call__(self, input_ids, attention_mask=None, token_type_ids=None, **unused) -> torch.Tensor:
         g = self.geometry
@@ -151,7 +142,7 @@ class BertTextEncoder:
         ids_d, len_d = ids.to(self.device), lengths.to(self.device)
         out = torch.empty(B, L, g["hidden"], device=self.device, dtype=torch.float32)
         capi.check(self.lib.ds_text_enc_forward(self.h, C.c_void_p(ids_d.data_ptr()), C.c_void_p(len_d.data_ptr()),
-                                                B, L, C.c_void_p(out.data_ptr()), self._stream()))
+                                                B, L, C.c_void_p(out.data_ptr()), capi.stream(self.device)))
         return out
 
     def close(self):
