@@ -24,6 +24,7 @@ TRAIN_COND = {n: i for i, n in enumerate((
     "dctx_act", "xkv", "xctx", "x_t"))}      # DS_TRAIN_COND indices (include/diffuscene_b200.h)
 ROOM_ENC_STATE = {n: i for i, n in enumerate((
     "x0", "a1", "p", "h", "o", "wp", "bias", "dwp", "dbias", "dz", "dh", "dp", "da1"))}      # DS_RE_* kinds
+TEXT_ENC_TAP = {n: i for i, n in enumerate(("x", "qkv", "ctx", "y1", "h1", "inter", "y2", "out"))}      # DS_TE_* kinds
 
 
 class DsConfig(C.Structure):
@@ -186,6 +187,8 @@ sig = {
     "ds_text_enc_expected_weight": (C.c_int, [_H, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64)]),
     "ds_text_enc_set_weights": (C.c_int, [_H, _p, _p]),
     "ds_text_enc_forward": (C.c_int, [_H, _p, _p, C.c_int32, C.c_int32, _p, _p]),
+    "ds_text_enc_set_tap": (C.c_int, [_H, C.c_int32]),
+    "ds_text_enc_read": (C.c_int, [_H, C.c_int32, _p, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _p]),
     "ds_vgg_create": (C.c_int, [C.POINTER(DsVggConfig), C.POINTER(_H)]),
     "ds_vgg_destroy": (C.c_int, [_H]),
     "ds_vgg_expected_weight_count": (C.c_int, [_H]),

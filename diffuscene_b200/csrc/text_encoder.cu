@@ -331,6 +331,7 @@ constexpr float TE_LN_EPS = 1e-12f;                 // BertConfig.layer_norm_eps
 constexpr int64_t TE_MAX_TOKENS = 65535LL * 64;     // the SIMT GEMM's gridDim.y (64 rows per CTA row)
 constexpr int TE_PER_LAYER = 16;                    // state-dict tensors per encoder layer
 enum { G_QKV = 0, G_OUT, G_INTER, G_FFN_OUT };
+constexpr int TE_TAPS = DS_TE_OUT + 1;
 }  // namespace
 
 struct ds_text_enc {
@@ -346,6 +347,11 @@ struct ds_text_enc {
   void *x = nullptr, *qkv = nullptr, *ctx = nullptr, *y = nullptr, *h1 = nullptr, *inter = nullptr;
   std::vector<GemmArgs> gemm;     // 4 per layer, M = capacity
   std::vector<TcGemmPlan*> tc;    // bf16: one plan per GEMM
+  // per-layer tap (ds_text_enc_set_tap): the tapped layer's arrays, storage type, one region per DS_TE_* kind
+  int tap_layer = -1;             // -1: off
+  void* tap = nullptr;            // allocated by the first ds_text_enc_set_tap, `capacity` tokens
+  int64_t tap_width[TE_TAPS] = {}, tap_off[TE_TAPS] = {};
+  int tapped_layer = -1, tapped_M = 0;      // layer and tokens of the last forward that ran with a tap set
 };
 
 namespace {
@@ -354,7 +360,7 @@ template <typename T> T* P(void* v, size_t off = 0) { return (T*)v + off; }
 void te_release(ds_text_enc* h) {
   for (auto* p : h->tc) if (p) tc_plan_destroy(p);
   h->tc.clear();
-  void* bufs[] = {h->params, h->wmat, h->bqkv, h->x, h->qkv, h->ctx, h->y, h->h1, h->inter};
+  void* bufs[] = {h->params, h->wmat, h->bqkv, h->x, h->qkv, h->ctx, h->y, h->h1, h->inter, h->tap};
   for (void* b : bufs) cudaFree(b);
   delete h;
 }
@@ -362,14 +368,25 @@ void te_release(ds_text_enc* h) {
 // flat offset of tensor `k` (0 .. 15, state-dict order) of layer `l`
 const float* layer_param(const ds_text_enc* h, const float* base, int l, int k) { return base + h->w.off[5 + TE_PER_LAYER * l + k]; }
 
+// copy `src` [M, width] of the tapped layer into the tap store (storage type)
+int te_tap(ds_text_enc* h, int l, int kind, const void* src, int M, cudaStream_t s) {
+  if (l != h->tap_layer) return 0;
+  const size_t n = (size_t)M * h->tap_width[kind] * h->esz;
+  const cudaError_t e = cudaMemcpyAsync((char*)h->tap + (size_t)h->tap_off[kind] * h->esz, src, n,
+                                        cudaMemcpyDeviceToDevice, s);
+  return e == cudaSuccess ? 0 : fail(DS_ERR_CUDA, "text encoder: tap copy failed: %s", cudaGetErrorString(e));
+}
+
 template <typename T>
 int te_forward(ds_text_enc* h, const int* ids, const int* lengths, int B, int L, float* out, cudaStream_t s) {
   const ds_text_enc_config& c = h->cfg;
   const int H = c.hidden, M = B * L;
   const float* pr = h->params;
+  h->tapped_layer = -1;
   launch_te_embed_ln<T>(ids, pr + h->w.off[0], pr + h->w.off[1], pr + h->w.off[2], pr + h->w.off[3], pr + h->w.off[4],
                         P<T>(h->x), M, L, H, c.vocab, TE_LN_EPS, s);
   for (int l = 0; l < c.layers; ++l) {
+    if (const int rc = te_tap(h, l, DS_TE_X, h->x, M, s)) return rc;
     for (int k = 0; k < 4; ++k) {
       const int gi = 4 * l + k;
       if (h->bf16) {
@@ -380,19 +397,34 @@ int te_forward(ds_text_enc* h, const int* ids, const int* lengths, int B, int L,
         g.M = M;
         launch_gemm_simt<float>(g, true, s);
       }
+      int rc = 0;
       if (k == G_QKV) {
+        rc = te_tap(h, l, DS_TE_QKV, h->qkv, M, s);
         launch_te_attention<T>(P<T>(h->qkv), lengths, P<T>(h->ctx), B, L, H, s);
+        if (!rc) rc = te_tap(h, l, DS_TE_CTX, h->ctx, M, s);
       } else if (k == G_OUT) {
+        rc = te_tap(h, l, DS_TE_Y1, h->y, M, s);
         launch_te_layernorm<T, T>(P<T>(h->y), layer_param(h, pr, l, 8), layer_param(h, pr, l, 9), P<T>(h->h1), M, H,
                                   TE_LN_EPS, s);
-      } else if (k == G_FFN_OUT) {
+        if (!rc) rc = te_tap(h, l, DS_TE_H1, h->h1, M, s);
+      } else if (k == G_INTER) {
+        rc = te_tap(h, l, DS_TE_INTER, h->inter, M, s);
+      } else {
+        rc = te_tap(h, l, DS_TE_Y2, h->y, M, s);
         const float* g = layer_param(h, pr, l, 14);
         const float* b = layer_param(h, pr, l, 15);
-        if (l + 1 < c.layers) launch_te_layernorm<T, T>(P<T>(h->y), g, b, P<T>(h->x), M, H, TE_LN_EPS, s);
-        else launch_te_layernorm<T, float>(P<T>(h->y), g, b, out, M, H, TE_LN_EPS, s);
+        if (l + 1 < c.layers) {
+          launch_te_layernorm<T, T>(P<T>(h->y), g, b, P<T>(h->x), M, H, TE_LN_EPS, s);
+          if (!rc) rc = te_tap(h, l, DS_TE_OUT, h->x, M, s);
+        } else {
+          launch_te_layernorm<T, float>(P<T>(h->y), g, b, out, M, H, TE_LN_EPS, s);
+        }
       }
+      if (rc) return rc;
     }
   }
+  h->tapped_layer = h->tap_layer;
+  h->tapped_M = h->tap_layer >= 0 ? M : 0;
   return 0;
 }
 
@@ -558,6 +590,51 @@ extern "C" int ds_text_enc_forward(ds_text_enc* h, const int32_t* ids_dev, const
   const int rc = h->bf16 ? te_forward<bf16>(h, ids_dev, lengths_dev, batch, seq_len, out_dev, s)
                          : te_forward<float>(h, ids_dev, lengths_dev, batch, seq_len, out_dev, s);
   if (rc) return rc;
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int ds_text_enc_set_tap(ds_text_enc* h, int32_t layer) {
+  if (!h) return fail(DS_ERR_INVALID, "null handle");
+  if (layer < -1 || layer >= h->cfg.layers)
+    return fail(DS_ERR_INVALID, "text encoder: tap layer %d outside [-1, %d)", layer, h->cfg.layers);
+  if (layer >= 0 && !h->tap) {
+    const int64_t H = h->cfg.hidden, w[TE_TAPS] = {H, 3 * H, H, H, H, h->cfg.intermediate, H, H};
+    int64_t total = 0;
+    for (int k = 0; k < TE_TAPS; ++k) {
+      h->tap_width[k] = w[k];
+      h->tap_off[k] = total * h->cfg.capacity;
+      total += w[k];
+    }
+    CK(cudaSetDevice(h->cfg.device));
+    const cudaError_t e = cudaMalloc(&h->tap, (size_t)total * h->cfg.capacity * h->esz);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      h->tap = nullptr;
+      return fail(DS_ERR_CUDA, "text encoder: tap store for %d tokens failed: %s", h->cfg.capacity, cudaGetErrorString(e));
+    }
+  }
+  h->tap_layer = layer;
+  return 0;
+}
+
+extern "C" int ds_text_enc_read(ds_text_enc* h, int32_t kind, float* dev_out, int64_t capacity, int32_t* rows,
+                                int32_t* width, void* stream) {
+  if (!h) return fail(DS_ERR_INVALID, "null handle");
+  if (h->tapped_layer < 0) return fail(DS_ERR_STATE, "text encoder: the last forward ran without a tap");
+  if (kind < 0 || kind >= TE_TAPS) return fail(DS_ERR_INVALID, "text encoder: bad tap kind %d", kind);
+  if (kind == DS_TE_OUT && h->tapped_layer == h->cfg.layers - 1)
+    return fail(DS_ERR_INVALID, "text encoder: the last layer's output is the forward's own output");
+  const int64_t r = h->tapped_M, w = h->tap_width[kind], n = r * w;
+  if (rows) *rows = int32_t(r);
+  if (width) *width = int32_t(w);
+  if (!dev_out) return 0;      // size query
+  if (n > capacity) return fail(DS_ERR_INVALID, "output capacity %lld < %lld", (long long)capacity, (long long)n);
+  CK(cudaSetDevice(h->cfg.device));
+  cudaStream_t s = (cudaStream_t)stream;
+  const void* src = (const char*)h->tap + (size_t)h->tap_off[kind] * h->esz;
+  if (h->bf16) launch_widen_bf16((const bf16*)src, dev_out, n, s);
+  else CK(cudaMemcpyAsync(dev_out, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
   CK(cudaGetLastError());
   return 0;
 }

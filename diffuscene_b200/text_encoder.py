@@ -115,6 +115,7 @@ class BertTextEncoder:
         self.lib = capi.load()
         self.h = C.c_void_p()
         self.capacity = 0
+        self.tap_layer = -1
         self._create(capacity)
 
     def _create(self, capacity: int):
@@ -129,6 +130,8 @@ class BertTextEncoder:
         self.h, self.capacity = h, capacity
         flat = self._flat_host.to(self.device)
         capi.check(self.lib.ds_text_enc_set_weights(self.h, C.c_void_p(flat.data_ptr()), capi.stream(self.device)))
+        if self.tap_layer >= 0:
+            capi.check(self.lib.ds_text_enc_set_tap(self.h, self.tap_layer))
 
     def expected_weights(self) -> List[Tuple[str, int]]:
         return capi.expected_weights(self.lib, "ds_text_enc", self.h)
@@ -143,6 +146,23 @@ class BertTextEncoder:
         out = torch.empty(B, L, g["hidden"], device=self.device, dtype=torch.float32)
         capi.check(self.lib.ds_text_enc_forward(self.h, C.c_void_p(ids_d.data_ptr()), C.c_void_p(len_d.data_ptr()),
                                                 B, L, C.c_void_p(out.data_ptr()), capi.stream(self.device)))
+        return out
+
+    def set_tap(self, layer: int):
+        """Tap encoder layer `layer` on the following forwards (ds_text_enc_set_tap); -1 turns the tap off."""
+        capi.check(self.lib.ds_text_enc_set_tap(self.h, int(layer)))
+        self.tap_layer = int(layer)
+
+    def read(self, kind) -> torch.Tensor:
+        """One array of the tapped layer of the last forward (ds_text_enc_read), fp32 [B * L, width] on the device:
+        kind is a name of capi.TEXT_ENC_TAP (or its DS_TE_* value)."""
+        if isinstance(kind, str):
+            kind = capi.TEXT_ENC_TAP[kind]
+        r, w = C.c_int32(), C.c_int32()
+        capi.check(self.lib.ds_text_enc_read(self.h, kind, None, 0, C.byref(r), C.byref(w), capi.stream(self.device)))
+        out = torch.empty(r.value, w.value, device=self.device, dtype=torch.float32)
+        capi.check(self.lib.ds_text_enc_read(self.h, kind, C.c_void_p(out.data_ptr()), out.numel(), C.byref(r),
+                                             C.byref(w), capi.stream(self.device)))
         return out
 
     def close(self):

@@ -629,6 +629,27 @@ DS_API int ds_text_enc_set_weights(ds_text_enc* h, const float* flat_params_dev,
  * above max_positions or batch x seq_len above the capacity. */
 DS_API int ds_text_enc_forward(ds_text_enc* h, const int32_t* ids_dev, const int32_t* lengths_dev, int32_t batch,
                                int32_t seq_len, float* out_dev, void* stream);
+/* Tap one encoder layer (test / profiling aid): while `layer` (0 .. layers - 1) is set, each forward also copies that
+ * layer's arrays, in the storage type, into a tap store on its stream; -1 (the default) turns the tap off, and the
+ * forward then launches nothing more.  The first call with a layer allocates the store for `capacity` tokens.
+ * DS_ERR_INVALID for a layer outside [-1, layers). */
+DS_API int ds_text_enc_set_tap(ds_text_enc* h, int32_t layer);
+/* Arrays of the tapped layer ds_text_enc_read copies (`kind`), rows [batch x seq_len] of the last forward:
+ *   DS_TE_X      the layer input x (for layer 0 the embedding LayerNorm output), [rows, hidden]
+ *   DS_TE_QKV    q | k | v = x [Wq | Wk | Wv]^T + [bq | bk | bv], [rows, 3 hidden]
+ *   DS_TE_CTX    the masked self-attention output, [rows, hidden]
+ *   DS_TE_Y1     ctx Wo^T + bo + x before its LayerNorm, [rows, hidden]
+ *   DS_TE_H1     LayerNorm(y1), [rows, hidden]
+ *   DS_TE_INTER  GELU(h1 W1^T + b1), [rows, intermediate]
+ *   DS_TE_Y2     inter W2^T + b2 + h1 before its LayerNorm, [rows, hidden]
+ *   DS_TE_OUT    the layer output LayerNorm(y2), [rows, hidden]; not for the last layer, whose output is the
+ *                forward's own fp32 output */
+enum { DS_TE_X = 0, DS_TE_QKV, DS_TE_CTX, DS_TE_Y1, DS_TE_H1, DS_TE_INTER, DS_TE_Y2, DS_TE_OUT };
+/* Copy one tapped array, widened to fp32, into dev_out [rows, width] on `stream`.  DS_ERR_STATE unless the last
+ * forward ran with a tap set; DS_ERR_INVALID for a bad kind (DS_TE_OUT of the last layer included) or capacity <
+ * rows * width floats.  dev_out == NULL: a size query, only rows and width are set. */
+DS_API int ds_text_enc_read(ds_text_enc* h, int32_t kind, float* dev_out, int64_t capacity, int32_t* rows,
+                            int32_t* width, void* stream);
 
 /* ---- improved precision and recall of rendered scenes ------------------------------------------
  * Feature extractor: torchvision `vgg16` as scripts/improved_precision_recall.py:159-163 (reference) uses it,

@@ -137,6 +137,13 @@ def test_batch_independence(precision):
     assert rel <= 1e-6
     # every kernel is row-wise or per sequence, and a sequence's keys stop at its length: extra padding changes no bit
     assert torch.equal(a, b)
+    # random tokens instead of [PAD] at every padded position: padded keys get exactly zero weight, so the valid
+    # positions keep every bit
+    noise = torch.randint(1, 1000, ids.shape, generator=torch.Generator().manual_seed(9))
+    ids_r = torch.where(mask.bool(), ids, noise)
+    assert (ids_r[~valid] != 0).all()
+    rand = enc(input_ids=ids_r, attention_mask=mask).cpu()
+    assert torch.equal(rand[valid], full[valid]), precision
     enc.close()
 
 
